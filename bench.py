@@ -1,5 +1,5 @@
 #!/usr/bin/env python3
-"""bench.py -- one JSON line per run (see the driver contract in the task statement).
+"""bench.py -- one JSON line per run.
 
 Workload (BASELINE.json configs[4], the one `metric` is quoted on): a synthetic NDJSON
 stream of parking-citations-shaped records (tests/golden/data/parking-citations.json.zst
@@ -13,11 +13,16 @@ every rank parses its own shard of the stream; record boundaries are shard bound
   e2e       same metric through the reference-facing call sj_parse() with HOST buffers:
             pinned host input -> H2D -> K1..K2f -> D2H of tape + strings, every step
   roofline  stage1_flatten kernel alone on the same batch: algorithmic bytes
-            (N_in + 4 * N_idx, SURVEY.md 8d) / CUDA-event time, against the measured HBM peak
+            (N_in + 4 * N_idx, SURVEY.md 8d) / CUDA-event time, against the H100 SXM data
+            sheet's 3.35 TB/s of HBM3 (a 700 W card; `clocks` names the card and its power limit)
   cpu_baseline / --impl reference
             the reference cannot be built here (no Go toolchain), so the CPU arm is the
             oracle port (C restatement; AVX-512BW mask routines when the host has them, else AVX2+PCLMUL) run
             ParseNDStream-style on all host threads (10 MiB newline-aligned chunks)
+
+--dump-outputs DIR writes what the timed device-resident step returned in its last step (tape and
+Strings.B, as exact float64 pieces plus a fixed seeded sample) so that two builds can be compared
+output for output on identical inputs.
 """
 import argparse
 import ctypes as C
@@ -34,8 +39,8 @@ sys.path.insert(0, os.path.join(ROOT, "simdjson-go_b200"))
 
 import numpy as np  # noqa: E402
 
-# BASELINE.json's metric, verbatim, in BOTH arms (the driver matches the two lines on it)
-METRIC = "GB/s JSON parsed end-to-end; stage1 achieved HBM GB/s vs B200 peak"
+# BASELINE.json's metric, verbatim, in BOTH arms (so the GPU line and the CPU line can be matched on it)
+METRIC = "GB/s JSON parsed end-to-end; stage1 achieved HBM GB/s vs H100 peak"
 WORKLOAD = ("synthetic NDJSON stream: parking-citations-shaped records (BASELINE configs[4]), ParseND, copy_strings=true")
 
 
@@ -71,11 +76,7 @@ def host_threads():
 
 
 def read_peaks():
-    try:
-        with open(os.path.join(ROOT, "MEASURED_PEAKS.json")) as f:
-            return float(json.load(f)["hbm_gbs"]), "measured"
-    except Exception:
-        return 6650.0, "fallback"
+    return 3350.0, "H100 SXM data sheet (700 W)"
 
 
 class ClockSampler(threading.Thread):
@@ -87,7 +88,7 @@ class ClockSampler(threading.Thread):
 
     def run(self):
         q = ("clocks.sm,clocks.max.sm,clocks_event_reasons.hw_slowdown,clocks_event_reasons.hw_thermal_slowdown,"
-             "clocks_event_reasons.sw_thermal_slowdown,clocks_event_reasons.sw_power_cap")
+             "clocks_event_reasons.sw_thermal_slowdown,clocks_event_reasons.sw_power_cap,name,power.limit")
         while not self.stop_flag:
             try:
                 out = subprocess.run(["nvidia-smi", "-i", str(self.index), "--query-gpu=" + q, "--format=csv,noheader,nounits"],
@@ -106,8 +107,10 @@ class ClockSampler(threading.Thread):
             for name, v in zip(("hw_slowdown", "hw_thermal_slowdown", "sw_thermal_slowdown", "sw_power_cap"), s[2:6]):
                 if v.lower().startswith("active"):
                     reasons.add(name)
+        last = self.samples[-1] if self.samples else []
         return {"sm_mhz": int(np.median(sm)) if sm else None, "sm_max_mhz": max(mx) if mx else None,
-                "reasons": sorted(reasons), "samples": len(sm)}
+                "reasons": sorted(reasons), "samples": len(sm), "gpu": last[6] if len(last) > 7 else None,
+                "power_limit_w": last[7] if len(last) > 7 else None}
 
 
 # --------------------------------------------------------------------------------------
@@ -201,15 +204,32 @@ def run_reference(args, rank, world):
 # --------------------------------------------------------------------------------------
 # GPU arm
 # --------------------------------------------------------------------------------------
-def k1_traffic(batch_bytes):
-    """dram__bytes_read.sum + dram__bytes_write.sum of ONE K1 launch on this batch, from the committed
-    `ncu --set full` capture of this very command (profiles/k1_traffic.json); None for other batch sizes."""
-    try:
-        with open(os.path.join(ROOT, "profiles", "k1_traffic.json")) as f:
-            t = json.load(f)
-        return t["dram_bytes_read"] + t["dram_bytes_write"] if int(t["batch_bytes"]) == int(batch_bytes) else None
-    except (OSError, ValueError, KeyError):
-        return None
+DUMP_SAMPLE = 1 << 20  # tape words and string bytes in the seeded sample of --dump-outputs
+
+
+def dump_outputs(outdir, tape, strings, suffix=""):
+    """What the device-resident step hands its caller -- Tape (uint64 words) and Strings.B (bytes) -- as float arrays
+    that hold them exactly: every tape word is split into its high and low 32 bits, summed per chunk of the tape
+    (float64 sums below 2^53 are exact, so the sums cover every word and byte), plus a fixed sample (seed 0) of words and string
+    bytes with their positions.  About 40 MB whatever the batch size."""
+    os.makedirs(outdir, exist_ok=True)
+    rng = np.random.default_rng(0)
+    chunks = 4096
+
+    def sums(x):
+        pad = (-len(x)) % chunks
+        return np.concatenate([x, np.zeros(pad, dtype=x.dtype)]).reshape(chunks, -1).astype(np.float64).sum(axis=1)
+
+    hi, lo = (tape >> np.uint64(32)).astype(np.uint32), (tape & np.uint64(0xFFFFFFFF)).astype(np.uint32)
+    ti = np.sort(rng.choice(len(tape), size=min(len(tape), DUMP_SAMPLE), replace=False))
+    si = np.sort(rng.choice(len(strings), size=min(len(strings), DUMP_SAMPLE), replace=False)) if len(strings) else np.zeros(0, np.int64)
+    out = {"tape_len": np.array([len(tape)], dtype=np.float64), "strings_len": np.array([len(strings)], dtype=np.float64),
+           "tape_hi_chunk_sums": sums(hi), "tape_lo_chunk_sums": sums(lo), "strings_chunk_sums": sums(strings),
+           "tape_sample_index": ti.astype(np.float64), "tape_sample_hi": hi[ti].astype(np.float64),
+           "tape_sample_lo": lo[ti].astype(np.float64), "strings_sample_index": si.astype(np.float64),
+           "strings_sample": strings[si].astype(np.float32)}
+    for name, a in out.items():
+        np.save(os.path.join(outdir, name + suffix + ".npy"), a)
 
 
 def main():
@@ -226,7 +246,8 @@ def main():
     ap.add_argument("--stream-ring-mib", type=int, default=1024, help="size of the pinned ring of generated records each rank cycles over")
     ap.add_argument("--stream-chunk-mib", type=int, default=256, help="chunk size of the library's stream pipeline")
     ap.add_argument("--nccl-exchange", action="store_true", help="N > 1: exchange the shard totals through NCCL even where the peer-memory kernel is available (A/B)")
-    ap.add_argument("--no-cpu", action="store_true", help="skip the cpu_baseline leg (profiling runs under ncu)")
+    ap.add_argument("--no-cpu", action="store_true", help="skip the cpu_baseline leg (profiling runs)")
+    ap.add_argument("--dump-outputs", metavar="DIR", help="write the last timed step's tape and Strings.B to DIR/<name>.npy")
     args = ap.parse_args()
     args.warmup = max(args.warmup, 3) if args.impl == "ours" else args.warmup
 
@@ -243,7 +264,7 @@ def main():
     from simdjson_b200 import _lib
 
     if not torch.cuda.is_available() or not sj.SupportedCPU():
-        raise SystemExit("bench.py: no CUDA sm_100 device -- the CUDA path has no CPU fallback")
+        raise SystemExit("bench.py: no CUDA sm_90 device -- the CUDA path has no CPU fallback")
     torch.cuda.set_device(local_rank)
     dev = torch.device("cuda", local_rank)
     if world > 1:
@@ -355,6 +376,9 @@ def main():
         assert b_host[1] == rank * tape_words and first == b_host[1] + (int(tape_h[0]) & ((1 << 56) - 1)), (b_host, first)
         if exchange == "nccl":
             L.sj_ctx_set_stream(ctx.h, None)
+    if args.dump_outputs:
+        dump_outputs(args.dump_outputs, d_tape[:tape_words].cpu().numpy().view(np.uint64), d_strings[:string_bytes].cpu().numpy(),
+                     "_rank%d" % rank if world > 1 else "")
 
     # ---- roofline: stage1_flatten alone on the same batch ----
     info = sj.Stage1Info()
@@ -615,8 +639,7 @@ def main():
                            "what": "the same sj_parse calls with WithCopyStrings(false) (options.go:13): the tape alone travels back"},
             "gpu_launches": int(launches),
             "roofline": {"bound": "hbm", "kernel": "stage1_flatten_kernel<ndjson>", "achieved": round(achieved, 2), "peak": peak,
-                         "unit": "GB/s", "frac": round(achieved / peak, 4), "peak_kind": peak_kind, "traffic": k1_traffic(n),
-                         "traffic_kind": "static: dram__bytes_read.sum + dram__bytes_write.sum of one K1 launch on this batch from the committed ncu --set full capture (profiles/k1_traffic.json, round 2), not measured in this run",
+                         "unit": "GB/s", "frac": round(achieved / peak, 4), "peak_kind": peak_kind,
                          "algorithmic_bytes_per_launch": alg_bytes, "ms_per_launch": round(t_s1 * 1e3, 4),
                          "input_read_gbs": round(n / t_s1 / 1e9, 2)},
             "roofline_parse": {"bound": "hbm", "what": "whole device-resident step (K1 + K2p/q/r + numbers, scope matching, links, roots), algorithmic bytes 2*N_in + 8*N_idx + 8*N_tape + N_strings (SURVEY.md 8d)",

@@ -1,5 +1,5 @@
 /*
- * simdjson_b200.h -- C ABI of the B200-native simdjson parse engine.
+ * simdjson_b200.h -- C ABI of the H100-native simdjson parse engine.
  *
  * This is the drop-in boundary for the ONE hot path of minio/simdjson-go that this
  * library replaces (SURVEY.md section 8b).  The reference has no FFI of its own
@@ -50,7 +50,7 @@ extern "C" {
 
 typedef struct sj_ctx sj_ctx;
 
-/* simdjson_amd64.go:37 SupportedCPU(): 1 when an sm_100 device is usable */
+/* simdjson_amd64.go:37 SupportedCPU(): 1 when an sm_90 device is usable */
 int sj_supported(void);
 int sj_device_count(void);
 const char* sj_error_string(int rc);

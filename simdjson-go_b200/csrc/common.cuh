@@ -1,5 +1,5 @@
 // common.cuh -- small PTX wrappers (mbarrier, 1-D TMA bulk copy, relaxed/volatile
-// global accesses) shared by the sm_100a kernels.  No CUTLASS/CUB dependency.
+// global accesses) shared by the sm_90a kernels.  No CUTLASS/CUB dependency.
 #pragma once
 #include <cstdint>
 #include <cuda_runtime.h>

@@ -93,9 +93,8 @@ SJ_HD bool atom_ok_fast(const uint8_t* img, uint32_t o, uint32_t avail, uint32_t
 // esc_decode for the common case -- "\\uXXXX" with four proper hex digits, not a surrogate, and nothing that looks like a
 // high surrogate six bytes in front of it -- straight from the step image with word accesses and register arithmetic
 // only: four aligned words cover the twelve bytes [o - 6, o + 6), funnel shifts align them, the hex digits are checked
-// and converted four at a time (SWAR).  No table look-ups: a first version that went through the 256-entry tables was
-// SLOWER than esc_decode (twitterescaped 65.7 -> 56.7 GB/s; two dependent shared-memory loads per digit in a kernel that
-// is bound by dependent latencies).  Returns false when it does not apply; esc_decode (s2s_core.h) is the definition and
+// and converted four at a time (SWAR).  No table look-ups: going through the 256-entry tables costs two dependent
+// shared-memory loads per digit in a kernel that is bound by dependent latencies.  Returns false when it does not apply; esc_decode (s2s_core.h) is the definition and
 // takes those cases -- including every digit quirk of parse_string_amd64.s:4-69, which is why only proper digits pass here.
 //   o: offset of the backslash in the image; avail: image bytes that are message bytes
 #ifndef SJ_S2S_ESC_UFAST
@@ -656,8 +655,7 @@ SJ_HD void s2s_slab(W& wp, const S2sParams& p, uint32_t slab, const S2sWarpMem& 
 
         // ---------------- the lane's events, in order ----------------
 #ifndef SJ_S2S_DIRECT_TAPE
-#define SJ_S2S_DIRECT_TAPE 1  // tape words go straight to global memory (0: staged in shared memory and copied out coalesced --
-                              // measured: twitter 218 -> 224 GB/s, twitterescaped 110 -> 113, gsoc-2018 267 -> 275, parking-citations the same)
+#define SJ_S2S_DIRECT_TAPE 1  // tape words go straight to global memory (0: staged in shared memory and copied out coalesced)
 #endif
         const bool staged = !SJ_S2S_DIRECT_TAPE && w_step <= S2S_TSTAGE_WORDS;  // warp-uniform
         const uint32_t slot0 = 1 + run.w;                // tape slot of the step's first word (slot 0: the first root word)

@@ -2,7 +2,7 @@
 //
 // Host logic here mirrors the reference's parse driver (parse_json_amd64.go:28-127) and
 // stage-1 driver epilogue (stage1_find_marks_amd64.go:115-148); all byte work runs in the
-// sm_100a kernels of stage1.cuh / stage2.cuh.  There is NO CPU fallback: without a CUDA
+// sm_90a kernels of stage1.cuh / stage2.cuh.  There is NO CPU fallback: without a CUDA
 // device every entry point returns SJ_ERR_NO_DEVICE.
 #include <chrono>
 #include <cstdio>
@@ -113,7 +113,7 @@ extern "C" int sj_supported(void) {
     int n = sj_device_count();
     for (int d = 0; d < n; d++) {
         cudaDeviceProp prop;
-        if (cudaGetDeviceProperties(&prop, d) == cudaSuccess && prop.major == 10) return 1;
+        if (cudaGetDeviceProperties(&prop, d) == cudaSuccess && prop.major == 9 && prop.minor == 0) return 1;
     }
     return 0;
 }
@@ -123,7 +123,7 @@ extern "C" const char* sj_error_string(int rc) {
     case SJ_OK: return "ok";
     case SJ_ERR_STAGE1: return "Failed to find all structural indices for stage 1";
     case SJ_ERR_STAGE2: return "Bad parsing while executing stage 2";
-    case SJ_ERR_NO_DEVICE: return "Host does not have a usable sm_100 CUDA device";
+    case SJ_ERR_NO_DEVICE: return "Host does not have a usable sm_90 CUDA device";
     case SJ_ERR_CAPACITY: return "output buffer too small";
     case SJ_ERR_TOO_LARGE: return "message too large for one call";
     case SJ_ERR_ARGUMENT: return "bad argument";
@@ -150,7 +150,7 @@ extern "C" int sj_ctx_create(int device, sj_ctx** out) {
     if (device >= n) return SJ_ERR_ARGUMENT;
     cudaDeviceProp prop;
     SJ_CUDA_CHECK(cudaGetDeviceProperties(&prop, device));
-    if (prop.major != 10) return SJ_ERR_NO_DEVICE;  // sm_100a-only binary
+    if (prop.major != 9 || prop.minor != 0) return SJ_ERR_NO_DEVICE;  // sm_90a-only binary
     SJ_CUDA_CHECK(cudaSetDevice(device));
     sj_ctx* c = new (std::nothrow) sj_ctx();
     if (!c) return SJ_ERR_ARGUMENT;

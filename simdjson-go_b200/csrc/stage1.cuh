@@ -1,5 +1,5 @@
 // stage1.cuh -- K1 `stage1_flatten`: structural-index discovery + flatten_bits as ONE
-// sm_100a kernel (the reference also fuses them: find_structural_bits_amd64.s:56-115).
+// sm_90a kernel (the reference also fuses them: find_structural_bits_amd64.s:56-115).
 //
 // Replaces, per 64-byte block (SURVEY.md 3.4):
 //   find_odd_backslash_sequences     find_odd_backslash_sequences_amd64.s:24-61
@@ -31,9 +31,8 @@ namespace sj {
 #define SJ_S1_WARPS 16
 #endif
 // Pause between two polls of a look-back (ns), and whether to pause before the first poll too.
-// With one descriptor slot per L2 line the chains are insensitive to both (0.50 ms per GiB with
-// no pause, 100 ns or 400 ns); with the descriptors of 128 tiles packed in one line a poll issued
-// while the other CTAs published cost microseconds (1.0 ms unless every look-back slept 1 us first).
+// With one descriptor slot per L2 line the chains are insensitive to both; with the descriptors
+// of 128 tiles packed in one line a poll issued while the other CTAs published cost microseconds.
 #ifndef SJ_SPIN_SLEEP
 #define SJ_SPIN_SLEEP 100
 #endif
@@ -249,7 +248,7 @@ __device__ __forceinline__ uint32_t bitsel(uint32_t m, uint32_t a, uint32_t b) {
 __device__ __forceinline__ void s2p_pair(uint32_t X, uint32_t Y, uint32_t m, int s, uint32_t& hi, uint32_t& lo) {
 #ifndef SJ_S2P_SHIFT
     // Y >> s as IMAD.HI: the classifier is bound by the ALU pipe (LOP3 / SHF / PRMT issue every
-    // other cycle), the FMA pipe is nearly idle -- measured 4 % faster than the SHF form
+    // other cycle), the FMA pipe is nearly idle
     hi = bitsel(m, X, __umulhi(Y, 1u << (32 - s)));
 #else
     hi = bitsel(m, X, Y >> s);
@@ -619,8 +618,8 @@ __device__ __forceinline__ void flatten_slab_staged(const uint64_t (&S)[STEPS], 
 // look-back chains over TILES (all slabs of one CTA iteration; only the scan warp of a CTA
 // publishes and polls).  Every tile owns one descriptor SLOT per chain, and the slots are
 // S1_DESC_STRIDE bytes apart, i.e. in different L2 lines: with the descriptors of 128 tiles packed
-// into one line (the previous layout) 148 CTAs published into and polled the same line at the
-// same moment, and a poll issued during that burst took microseconds.
+// into one line (the previous layout) every CTA of the grid published into and polled the same line
+// at the same moment, and a poll issued during that burst took microseconds.
 //   chain 1 (in-string parity): uint32 {bit0 valid, bit1 inclusive, bit2 parity}
 //   chain 2 (structural count): 16 bytes {uint32 aggregate | bit31 valid, pad, uint64 inclusive
 //            prefix | bit63 valid}

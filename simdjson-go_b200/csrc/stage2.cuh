@@ -39,7 +39,7 @@ constexpr uint32_t S2_COOP_MIN = SJ_S2_COOP_MIN;  // 0xffffffff: never (thread-s
 #define SJ_S2_DENSE_NUMBERS 1
 #endif
 constexpr bool S2_DENSE_NUMBERS = SJ_S2_DENSE_NUMBERS != 0;  // number-heavy documents: numbers parsed by their own dense kernel
-// tuning knobs for `tools/gpu_checks.sh` variants (build_variants/*.so); the defaults are the measured configuration
+// tuning knobs for variant builds (tools/build_variants.sh -> build_variants/*.so)
 #ifndef SJ_S2_DENSE_NUMBERS_SHIFT
 #define SJ_S2_DENSE_NUMBERS_SHIFT 4  // dense kernels when numbers << SHIFT >= structurals (one structural in 16)
 #endif
@@ -53,14 +53,13 @@ constexpr bool S2_DENSE_NUMBERS = SJ_S2_DENSE_NUMBERS != 0;  // number-heavy doc
 #define SJ_S2_FAST_ESCAPES 1
 #endif
 constexpr bool S2_FAST_ESCAPES = SJ_S2_FAST_ESCAPES != 0;  // warp routines decode all escapes of a window at once (warp_string_fast)
-// K2c (unescape): windows with one or two backslashes take the exact step -- measured: twitter 224 -> 215 us,
-// twitterescaped 532 -> 556 us per 64 MiB against decoding every window.  K2a (measure): see SJ_S2_FAST_MEASURE.
+// K2c (unescape): windows with one or two backslashes take the exact step instead of decoding every window.
+// K2a (measure): see SJ_S2_FAST_MEASURE.
 #ifndef SJ_S2_FAST_MIN_BACKSLASHES
 #define SJ_S2_FAST_MIN_BACKSLASHES 3
 #endif
-// K2a's long-string measure: 0 = exact warp routine, 1 = warp_string_fast inlined, 2 = warp_string_fast behind a call
-// measured (twitter / twitterescaped / gsoc-2018, GB/s per 256 MiB document): 0: 157.5 / 37.3 / 178.3,
-// 1: 131.7 / 48.5 / 168.0 (the inlined routine changes the code of the whole kernel), 2: 152.6 / 60.5 / 173.1
+// K2a's long-string measure: 0 = exact warp routine, 1 = warp_string_fast inlined (the inlined routine changes the
+// code of the whole kernel), 2 = warp_string_fast behind a call
 #ifndef SJ_S2_FAST_MEASURE
 #define SJ_S2_FAST_MEASURE 2
 #endif
@@ -947,7 +946,7 @@ __global__ void __launch_bounds__(1024) s2_scan_top_kernel(const ScanVal* in, ui
 // K2c
 // ---------------------------------------------------------------------------------
 // One structural per thread, warps independent of each other: with four structurals per thread the
-// tape stores of a warp spread over 32 sectors and the kernel got slower (541 -> 640 us).
+// tape stores of a warp spread over 32 sectors.
 __global__ void __launch_bounds__(S2_THREADS, SJ_S2_EMIT_MIN_BLOCKS) s2_emit_kernel(const Stage2Params p) {  // 8 blocks per SM = 32 registers: the kernel hides its load latency with occupancy
     const uint32_t i = blockIdx.x * S2_THREADS + threadIdx.x;
     const uint32_t lane = threadIdx.x & 31;

@@ -2,7 +2,7 @@
 
 // Package simdjson: drop-in replacement for parse_json_amd64.go of minio/simdjson-go.
 //
-// This file is the ONLY Go code the B200 path needs: it replaces
+// This file is the ONLY Go code the GPU path needs: it replaces
 // (*internalParsedJson).parseMessage (reference parse_json_amd64.go:52) with one cgo call into
 // libsimdjson_b200.so.  Parse / ParseND / ParseNDStream (simdjson_amd64.go:66,82,116) and every
 // tape consumer (Iter, Object, Array, Serializer) stay as they are: the {Message, Tape,
@@ -53,7 +53,7 @@ func b200Put(h *C.sj_ctx) {
 	}
 }
 
-// SupportedCPU reports whether the B200 path can run (simdjson_amd64.go:37).
+// SupportedCPU reports whether the GPU path can run (simdjson_amd64.go:37).
 func SupportedCPU() bool { return C.sj_supported() != 0 }
 
 func (pj *internalParsedJson) parseMessage(msg []byte, ndjson bool) error {

@@ -2,7 +2,7 @@
 
 Names follow the reference (minio/simdjson-go): SupportedCPU (simdjson_amd64.go:37),
 Parse (:66), ParseND (:82), ParsedJson{Message, Tape, Strings} (parsed_json.go:64-71),
-WithCopyStrings (options.go:13).  All byte work happens in the sm_100a kernels behind
+WithCopyStrings (options.go:13).  All byte work happens in the sm_90a kernels behind
 libsimdjson_b200.so; this module only marshals buffers.  No CPU fallback.
 """
 import ctypes as C
@@ -19,7 +19,7 @@ M64 = (1 << 64) - 1
 
 
 def SupportedCPU():
-    """simdjson_amd64.go:37 -- here: is an sm_100 device usable?"""
+    """simdjson_amd64.go:37 -- here: is an sm_90 device usable?"""
     return bool(_lib.load().sj_supported())
 
 

@@ -1,8 +1,8 @@
 """ctypes binding of the C ABI declared in include/simdjson_b200.h.
 
-The shared library is built in-tree by __graft_entry__.build() (nvcc, sm_100a) as
+The shared library is built in-tree by __graft_entry__.build() (nvcc, sm_90a) as
 simdjson-go_b200/libsimdjson_b200.so.  There is no CPU fallback: loading fails loudly if
-the library is missing, and every call fails with SJ_ERR_NO_DEVICE without a B200.
+the library is missing, and every call fails with SJ_ERR_NO_DEVICE without an H100.
 """
 import ctypes as C
 import os
@@ -50,7 +50,7 @@ def load():
         return _lib
     if not os.path.exists(LIB_PATH):
         raise RuntimeError("simdjson_b200: %s is missing -- run `python -c 'import __graft_entry__ as g; g.build()'` "
-                           "(nvcc, sm_100a); there is no CPU fallback" % LIB_PATH)
+                           "(nvcc, sm_90a); there is no CPU fallback" % LIB_PATH)
     L = C.CDLL(LIB_PATH)
     vp, sz, u32, u64, i32 = C.c_void_p, C.c_size_t, C.c_uint32, C.c_uint64, C.c_int
     szp = C.POINTER(C.c_size_t)

@@ -1,10 +1,9 @@
 #!/usr/bin/env python3
 """Extract the reference's golden vectors into JSON fixtures.
 
-Run in the BUILD container only (it reads /root/reference, which does not exist
-on the GPU box):
+Run it where a checkout of minio/simdjson-go is at hand; the tests only read its output:
 
-    python tests/golden/make_golden.py
+    python tests/golden/make_golden.py <path of the simdjson-go checkout>
 
 It parses the table-driven test literals out of the reference's Go test files
 with a small Go-literal evaluator (raw/interpreted strings, rune and integer
@@ -12,7 +11,7 @@ literals, composite literals with positional or keyed fields, a handful of
 conversions) and writes tests/golden/*.json. Byte strings are stored as hex so
 that control characters and invalid UTF-8 survive. It also copies the
 reference's compressed data fixtures (testdata/*.zst: public JSON corpora, data
-not source) to tests/golden/data/ so the GPU box has them.
+not source) to tests/golden/data/, so the tests need nothing outside this repository.
 
 Golden-vector ids (G1..G20) follow SURVEY.md appendix D.
 """
@@ -22,7 +21,7 @@ import re
 import shutil
 import sys
 
-REF = "/root/reference"
+REF = sys.argv[1] if __name__ == "__main__" and len(sys.argv) > 1 else "simdjson-go"
 OUT = os.path.dirname(os.path.abspath(__file__))
 
 

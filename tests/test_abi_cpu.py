@@ -99,4 +99,4 @@ def test_header_is_plain_c_and_links_from_c(lib, tmp_path):
     out = subprocess.run([exe], capture_output=True, text=True, timeout=120)
     assert "trimmed window: [1, 49)" in out.stdout, out.stdout + out.stderr
     if not torch.cuda.is_available():
-        assert out.returncode == 3 and "no sm_100 device" in out.stdout, out.stdout + out.stderr
+        assert out.returncode == 3 and "no sm_90 device" in out.stdout, out.stdout + out.stderr

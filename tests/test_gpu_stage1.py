@@ -16,7 +16,7 @@ M64 = (1 << 64) - 1
 def ctx():
     import simdjson_b200 as sj
     if not sj.SupportedCPU():
-        pytest.skip("no sm_100 device (the CUDA path has no CPU fallback)")
+        pytest.skip("no sm_90 device (the CUDA path has no CPU fallback)")
     c = sj.Context(0)
     yield c
     c.close()

@@ -1,6 +1,6 @@
 """World-size-2 gloo test of the N > 1 path's host logic (CPU only): newline-aligned
 sharding, the 3-integer all_gather, and tape rebasing.  Shards are parsed with the CPU oracle
-here (no GPU in this container); on the GPU box the same code runs over NCCL in bench.py."""
+here (no GPU needed); on GPUs the same code runs over NCCL in bench.py."""
 import os
 import socket
 import sys
@@ -90,7 +90,7 @@ def test_split_at_newlines_covers_and_aligns():
 
 
 def test_bench_reference_arm_prints_the_contract_line():
-    """bench.py --impl reference (the CPU arm of the driver's ratio) runs without a GPU and prints one
+    """bench.py --impl reference (the CPU arm the GPU line is compared with) runs without a GPU and prints one
     JSON line with the contract's keys"""
     import json
     import subprocess

@@ -1,6 +1,6 @@
 /* abi_example.c -- the C ABI used from plain C (what a cgo / JNI / FFI binding sees): compiled as C11 by the
  * CPU test-suite to prove that include/simdjson_b200.h is a C header and that the library links without any
- * C++ or CUDA types in the signatures.  Exit code 3 (SJ_ERR_NO_DEVICE) on a machine without an sm_100 GPU:
+ * C++ or CUDA types in the signatures.  Exit code 3 (SJ_ERR_NO_DEVICE) on a machine without an sm_90 GPU:
  * there is no CPU fallback.
  *   gcc -std=c11 -Wall -Wextra -Werror -Iinclude tools/abi_example.c -Lsimdjson-go_b200 -lsimdjson_b200 \
  *       -Wl,-rpath,$PWD/simdjson-go_b200 -o /tmp/abi_example */
@@ -18,7 +18,7 @@ int main(void) {
     if (!sj_supported()) {
         sj_ctx* none = NULL;
         int rc = sj_ctx_create(0, &none);
-        printf("no sm_100 device: sj_ctx_create -> %d (%s)\n", rc, sj_error_string(rc));
+        printf("no sm_90 device: sj_ctx_create -> %d (%s)\n", rc, sj_error_string(rc));
         return rc;
     }
     sj_ctx* ctx = NULL;

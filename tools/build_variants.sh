@@ -9,7 +9,7 @@ set -eu
 cd "$(dirname "$0")/.."
 OUT=${SJ_VARIANT_DIR:-build_variants}
 mkdir -p "$OUT"
-F="-gencode arch=compute_100a,code=sm_100a -O3 -lineinfo -std=c++17 -shared -Xcompiler -fPIC"
+F="-gencode arch=compute_90a,code=sm_90a -O3 -lineinfo -std=c++17 -shared -Xcompiler -fPIC"
 pids=()
 for spec in "$@"; do
   name=${spec%%=*}

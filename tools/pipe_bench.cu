@@ -1,5 +1,5 @@
 // Development aid: issue throughput of the integer instructions K1 is made of (per SM sub-partition).
-// nvcc -gencode arch=compute_100a,code=sm_100a -O3 -o pipe_bench tools/pipe_bench.cu
+// nvcc -gencode arch=compute_90a,code=sm_90a -O3 -o pipe_bench tools/pipe_bench.cu
 #include <cstdio>
 #include <cstdint>
 #include <cuda_runtime.h>
