@@ -229,17 +229,13 @@ SJ_HD uint64_t range64(uint32_t lo, uint32_t hi) { return lo >= hi ? 0ull : belo
 // geometry (the slab is the stage-1 kernel's slab: K1 hands over the in-string state in front of each one)
 // ---------------------------------------------------------------------------------
 constexpr uint32_t S2S_STEP_BYTES = 2048;                            // one warp pass: 32 lanes x 64 bytes
-#ifndef SJ_S1_STEPS
-#define SJ_S1_STEPS 3
-#endif
-constexpr uint32_t S2S_STEPS = SJ_S1_STEPS;  // 2 KiB steps per slab, the same in stage 1 (its in-string bits are per slab)
+constexpr uint32_t S2S_STEPS = 3;  // 2 KiB steps per slab; stage 1 uses the same (S1_STEPS): its in-string bits are per slab
 constexpr uint32_t S2S_SLAB_BYTES = S2S_STEPS * S2S_STEP_BYTES;      // == S1_SLAB_BYTES (static_assert in stage2_stream.cuh)
 constexpr uint32_t S2S_IMAGE_BYTES = 2 * S2S_STEP_BYTES;              // two image buffers: the step at hand and the next one in flight
 constexpr uint32_t S2S_SSTAGE_BYTES = S2S_STEP_BYTES + 32;           // compacted string bytes of one step (+ alignment shift)
-#ifndef SJ_S2S_TSTAGE_WORDS
-#define SJ_S2S_TSTAGE_WORDS 640
-#endif
-constexpr uint32_t S2S_TSTAGE_WORDS = SJ_S2S_TSTAGE_WORDS;                           // tape words of one step staged in shared memory (denser steps go straight to global memory)
+// K2r's tape-staging area (8-byte words), which holds the escape scratch: more than the escapes need, and its size is
+// part of K2r's shared memory per block, so it sets K2r's occupancy
+constexpr uint32_t S2S_TSTAGE_WORDS = 640;
 
 // per-slab aggregate (K2p) / exclusive prefix (K2q).  `trail`: string-buffer bytes behind the last real quote of
 // the slab (all of them if the slab holds no quote) -- scanned with the segmented operator below it gives, for a
@@ -583,11 +579,11 @@ SJ_HD uint64_t s2s_str_base(const S2sParams& p) { return p.bases_dev ? p.bases_d
 struct S2sWarpMem {
     uint8_t* src;        // [S2S_IMAGE_BYTES] two step images, 16-byte chunks XOR-swizzled inside each 64-byte block pair
     uint8_t* sstage;     // [S2S_SSTAGE_BYTES] compacted string bytes of the current step
-    uint64_t* tstage;    // [S2S_TSTAGE_WORDS] tape words of the current step
+    uint64_t* tstage;    // [S2S_TSTAGE_WORDS] K2r's tape-staging area (esc points into it)
     const uint8_t* ctab;   // [256] char_type
     const uint8_t* oktab;  // [256] transition_mask(p, c) at [p * 16 + c]
     const uint32_t* cmptab;  // [16] compress_sel(m) | popcount(m) << 16
-    uint8_t* esc;            // [S2S_ESC_SCRATCH] drop map + list of a step's escapes (K2r: the tape staging area, idle then)
+    uint8_t* esc;            // [S2S_ESC_SCRATCH] drop map + list of a step's escapes (K2r: the tape-staging area)
 };
 // scratch of a step's escapes: the drop map (one bit per image byte + one word behind the step), the record of the escape
 // whose output runs past the end of the step, the list of escape positions (an escape is at least two bytes long)

@@ -97,11 +97,8 @@ SJ_HD bool atom_ok_fast(const uint8_t* img, uint32_t o, uint32_t avail, uint32_t
 // shared-memory loads per digit in a kernel that is bound by dependent latencies.  Returns false when it does not apply; esc_decode (s2s_core.h) is the definition and
 // takes those cases -- including every digit quirk of parse_string_amd64.s:4-69, which is why only proper digits pass here.
 //   o: offset of the backslash in the image; avail: image bytes that are message bytes
-#ifndef SJ_S2S_ESC_UFAST
-#define SJ_S2S_ESC_UFAST 1
-#endif
 SJ_HD bool esc_u_fast(const uint8_t* img, uint32_t o, uint32_t avail, EscInfo& r) {
-    if (!SJ_S2S_ESC_UFAST || o < 6 || o + 6 > avail) return false;
+    if (o < 6 || o + 6 > avail) return false;
     const uint32_t a = (o - 6) & ~3u, sh = 8 * ((o - 6) & 3u);
     const uint32_t a3 = a + 12 < S2S_STEP_BYTES ? a + 12 : a + 8;  // (the fourth word only matters when sh != 0, and then it is inside)
     const uint32_t w0 = *reinterpret_cast<const uint32_t*>(img + swz(a)), w1 = *reinterpret_cast<const uint32_t*>(img + swz(a + 4));
@@ -653,13 +650,8 @@ SJ_HD void s2s_slab(W& wp, const S2sParams& p, uint32_t slab, const S2sWarpMem& 
             }
         }
 
-        // ---------------- the lane's events, in order ----------------
-#ifndef SJ_S2S_DIRECT_TAPE
-#define SJ_S2S_DIRECT_TAPE 1  // tape words go straight to global memory (0: staged in shared memory and copied out coalesced)
-#endif
-        const bool staged = !SJ_S2S_DIRECT_TAPE && w_step <= S2S_TSTAGE_WORDS;  // warp-uniform
+        // ---------------- the lane's events, in order (tape words go straight to global memory) ----------------
         const uint32_t slot0 = 1 + run.w;                // tape slot of the step's first word (slot 0: the first root word)
-        uint64_t* tout = staged ? sm.tstage - slot0 : p.tape;
         {
             // refined type of the last event in front of the lane
             const uint32_t nev = pi::popc64(EV);
@@ -747,7 +739,7 @@ SJ_HD void s2s_slab(W& wp, const S2sParams& p, uint32_t slab, const S2sWarpMem& 
                         p.brk_tp[kb] = slot;
                         p.brk_depth[kb] = depth_b + (int32_t)pi::popc32(opn & lo) - (int32_t)pi::popc32(brk & ~opn & lo);
                         p.brk_kind[kb] = (uint8_t)(opening ? (curly ? T_OBJ_OPEN : T_ARR_OPEN) : (curly ? T_OBJ_CLOSE : T_ARR_CLOSE));
-                        tout[slot] = (uint64_t)((opening ? 0x5bu : 0x5du) | (curly ? 0x20u : 0u)) << 56;  // payload cross-linked after the scope matching
+                        p.tape[slot] = (uint64_t)((opening ? 0x5bu : 0x5du) | (curly ? 0x20u : 0u)) << 56;  // payload cross-linked after the scope matching
                         const uint32_t seg = upto & ~prevm;
                         const uint32_t bad = segbad | ((bdr & seg) ? 1u : 0u) | ((bdo & seg) ? 2u : 0u) | ((bda & seg) ? 4u : 0u);
                         if (bad) wp.atomic_and(p.segmask + (kb >> 2), ~(bad << (8 * (kb & 3))));
@@ -764,8 +756,8 @@ SJ_HD void s2s_slab(W& wp, const S2sParams& p, uint32_t slab, const S2sWarpMem& 
                     const uint32_t kbelow = pi::popc32(kk & lo);
                     const uint32_t lower = qq & lo;  // the opening quote is the highest quote below, if it is in this half
                     const uint32_t dl = lower ? pi::popc32(kk & lo & ~((1u << (31 - pi::clz32(lower))) - 1u)) : pre_dl + kbelow;
-                    tout[slot] = ((uint64_t)'"' << 56) | (STRINGBUFBIT + out_str_base + (uint64_t)(lane_str + rank_b + kbelow - dl));
-                    tout[slot + 1] = dl;
+                    p.tape[slot] = ((uint64_t)'"' << 56) | (STRINGBUFBIT + out_str_base + (uint64_t)(lane_str + rank_b + kbelow - dl));
+                    p.tape[slot + 1] = dl;
                 }
                 // numbers: parsed by K2h from the list
                 for (uint32_t mm = num; mm; mm &= mm - 1) {
@@ -786,7 +778,7 @@ SJ_HD void s2s_slab(W& wp, const S2sParams& p, uint32_t slab, const S2sWarpMem& 
                         ok = atom_ok_p(rd, half_pos + j, p.len, sm.ctab[ch]);
                     }
                     if (!ok) err = 1;
-                    tout[slot] = (uint64_t)ch << 56;
+                    p.tape[slot] = (uint64_t)ch << 56;
                 }
                 // totals of the half
                 const uint32_t nk = pi::popc32(kk), nopn = pi::popc32(opn), nbr = pi::popc32(brk);
@@ -801,13 +793,7 @@ SJ_HD void s2s_slab(W& wp, const S2sParams& p, uint32_t slab, const S2sWarpMem& 
             // the segment behind the lane's last bracket goes on in the next lanes
             if (segbad) wp.atomic_and(p.segmask + (kb_b >> 2), ~(segbad << (8 * (kb_b & 3))));
         }
-        if (staged) {
-            wp.sync();
-            uint64_t* dst = p.tape + slot0;
-            for (uint32_t i = lane; i < w_step; i += 32) dst[i] = sm.tstage[i];
-            wp.sync();
-        }
-        wp.sync();  // both staging areas are reused by the next step
+        wp.sync();  // the string staging area and the escape scratch are reused by the next step
         run.w += w_step;
         run.str += k_step;
         run.brk += b_step;

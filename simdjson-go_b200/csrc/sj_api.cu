@@ -156,10 +156,6 @@ extern "C" int sj_ctx_create(int device, sj_ctx** out) {
     if (!c) return SJ_ERR_ARGUMENT;
     c->device = device;
     c->sm_count = prop.multiProcessorCount;
-    {
-        const char* e = getenv("SJ_B200_STAGE2");
-        c->s2_impl = (e && strcmp(e, "legacy") == 0) ? 1 : 0;
-    }
     // every failure below leaves through sj_ctx_destroy (stream, events, pinned result block, device scratch)
     const int rc = [&]() -> int {
         SJ_CUDA_CHECK(cudaStreamCreateWithFlags(&c->own_stream, cudaStreamNonBlocking));
@@ -213,7 +209,7 @@ extern "C" void sj_ctx_destroy(sj_ctx* c) {
 }
 
 // stage-2 implementation of a context: 0 = streaming kernels when copy_strings is on (default), 1 = per-structural
-// kernels always.  The environment variable SJ_B200_STAGE2=legacy selects 1 for every new context (A/B runs).
+// kernels always (the tests check the streaming kernels against them).
 extern "C" int sj_ctx_set_stage2_impl(sj_ctx* c, int impl) {
     if (!c || impl < 0 || impl > 1) return SJ_ERR_ARGUMENT;
     c->s2_impl = impl;

@@ -24,31 +24,18 @@
 // planes + Boolean class functions) instead of per-byte compares.
 #pragma once
 #include "common.cuh"
+#include "s2s_core.h"
 
 namespace sj {
 
-#ifndef SJ_S1_WARPS
-#define SJ_S1_WARPS 16
-#endif
-// Pause between two polls of a look-back (ns), and whether to pause before the first poll too.
-// With one descriptor slot per L2 line the chains are insensitive to both; with the descriptors
-// of 128 tiles packed in one line a poll issued while the other CTAs published cost microseconds.
-#ifndef SJ_SPIN_SLEEP
-#define SJ_SPIN_SLEEP 100
-#endif
-#ifndef SJ_SPIN_FIRST
-#define SJ_SPIN_FIRST 0
-#endif
-#ifndef SJ_S1_CTAS_PER_SM
-#define SJ_S1_CTAS_PER_SM 1
-#endif
-constexpr int S1_WARPS = SJ_S1_WARPS;            // warps per CTA = slabs per tile
-constexpr int S1_CTAS_PER_SM = SJ_S1_CTAS_PER_SM;
+constexpr int S1_WARPS = 16;                     // warps per CTA = slabs per tile
+// Pause between two polls of a look-back (ns); the first poll is not preceded by one.  With one descriptor slot per
+// L2 line the chains are insensitive to it; with the descriptors of 128 tiles packed in one line a poll issued while
+// the other CTAs published cost microseconds.
+constexpr unsigned S1_SPIN_SLEEP_NS = 100;
+constexpr int S1_CTAS_PER_SM = 1;
 constexpr int S1_THREADS = (S1_WARPS + 1) * 32;  // worker warps + one scan warp (the look-backs)
-#ifndef SJ_S1_STEPS
-#define SJ_S1_STEPS 3
-#endif
-constexpr int S1_STEPS = SJ_S1_STEPS;            // 2 KiB steps per slab
+constexpr int S1_STEPS = (int)S2S_STEPS;         // 2 KiB steps per slab (the streaming stage 2 walks the same slabs)
 constexpr int S1_STEP_BYTES = 32 * 64;
 constexpr int S1_SLAB_BYTES = S1_STEPS * S1_STEP_BYTES;  // 6 KiB per warp
 constexpr int S1_TILE_BYTES = S1_WARPS * S1_SLAB_BYTES;  // one look-back per tile
@@ -246,13 +233,9 @@ __device__ __forceinline__ uint32_t bitsel(uint32_t m, uint32_t a, uint32_t b) {
     return d;
 }
 __device__ __forceinline__ void s2p_pair(uint32_t X, uint32_t Y, uint32_t m, int s, uint32_t& hi, uint32_t& lo) {
-#ifndef SJ_S2P_SHIFT
     // Y >> s as IMAD.HI: the classifier is bound by the ALU pipe (LOP3 / SHF / PRMT issue every
     // other cycle), the FMA pipe is nearly idle
     hi = bitsel(m, X, __umulhi(Y, 1u << (32 - s)));
-#else
-    hi = bitsel(m, X, Y >> s);
-#endif
     lo = bitsel(m, X << s, Y);
 }
 
@@ -376,9 +359,7 @@ __device__ __forceinline__ uint64_t finalize_structurals(uint64_t st, uint64_t w
 // ---------------------------------------------------------------------------------
 // `stage` (optional): stage_cap x uint32 of shared memory private to the warp; the lanes drop their
 // entries there and the warp then streams them out with fully coalesced 128-byte stores.
-#ifndef SJ_FLATTEN_UNROLL
-#define SJ_FLATTEN_UNROLL 2
-#endif
+constexpr int S1_FLATTEN_UNROLL = 2;  // positions per half and trip of the extraction loops
 // index of the highest set bit (0xffffffff for 0): one FLO
 __device__ __forceinline__ uint32_t bfind(uint32_t x) {
     uint32_t b;
@@ -436,7 +417,7 @@ __device__ __forceinline__ uint32_t flatten_step(uint64_t S, uint32_t blockpos, 
         // (an exhausted half never uses its cursor again, so the cursors advance unconditionally)
         while (lo | hi) {
 #pragma unroll
-            for (int u = 0; u < SJ_FLATTEN_UNROLL; u++) {
+            for (int u = 0; u < S1_FLATTEN_UNROLL; u++) {
                 {
                     const uint32_t p = pos0 + (__ffs(lo) - 1);
                     sts_if(alo + 4 * u, DELTAS ? p - prev : p, lo);
@@ -450,8 +431,8 @@ __device__ __forceinline__ uint32_t flatten_step(uint64_t S, uint32_t blockpos, 
                     hi &= hi - 1;
                 }
             }
-            alo += 4 * SJ_FLATTEN_UNROLL;
-            ahi += 4 * SJ_FLATTEN_UNROLL;
+            alo += 4 * S1_FLATTEN_UNROLL;
+            ahi += 4 * S1_FLATTEN_UNROLL;
         }
         __syncwarp();
         for (uint32_t k = lane; k < total; k += 32) out[base + k] = stage[k];
@@ -499,7 +480,7 @@ __device__ __forceinline__ uint32_t extract_step(uint64_t S, uint32_t pos0, uint
     const uint32_t pos1 = pos0 + 32;
     while (lo | hi) {
 #pragma unroll
-        for (int u = 0; u < SJ_FLATTEN_UNROLL; u++) {
+        for (int u = 0; u < S1_FLATTEN_UNROLL; u++) {
             {
                 const uint32_t b = bfind(lo);
                 sts_if(alo - 4 * u, pos0 + b, lo);
@@ -511,8 +492,8 @@ __device__ __forceinline__ uint32_t extract_step(uint64_t S, uint32_t pos0, uint
                 hi &= ~(1u << (b & 31));
             }
         }
-        alo -= 4 * SJ_FLATTEN_UNROLL;
-        ahi -= 4 * SJ_FLATTEN_UNROLL;
+        alo -= 4 * S1_FLATTEN_UNROLL;
+        ahi -= 4 * S1_FLATTEN_UNROLL;
     }
     return total;
 }
@@ -594,7 +575,7 @@ __device__ __forceinline__ void flatten_slab_staged(const uint64_t (&S)[STEPS], 
         uint32_t alo = ahi - 4 * ch;
         while (lo | hi) {
 #pragma unroll
-            for (int u = 0; u < SJ_FLATTEN_UNROLL; u++) {
+            for (int u = 0; u < S1_FLATTEN_UNROLL; u++) {
                 {
                     const uint32_t b = bfind(lo);
                     sts_if(alo - 4 * u, pos0 + b, lo);
@@ -606,8 +587,8 @@ __device__ __forceinline__ void flatten_slab_staged(const uint64_t (&S)[STEPS], 
                     hi &= ~(1u << (b & 31));
                 }
             }
-            alo -= 4 * SJ_FLATTEN_UNROLL;
-            ahi -= 4 * SJ_FLATTEN_UNROLL;
+            alo -= 4 * S1_FLATTEN_UNROLL;
+            ahi -= 4 * S1_FLATTEN_UNROLL;
         }
         so += total;
     }
@@ -627,10 +608,7 @@ __device__ __forceinline__ void flatten_slab_staged(const uint64_t (&S)[STEPS], 
 // flight at once; with a grid of at most 32 * S1_LB_PER_LANE CTAs the tile this CTA published
 // one iteration ago (always inclusive) is inside the first round.
 // ---------------------------------------------------------------------------------
-#ifndef SJ_S1_DESC_STRIDE
-#define SJ_S1_DESC_STRIDE 128
-#endif
-constexpr int S1_DESC_STRIDE = SJ_S1_DESC_STRIDE;
+constexpr int S1_DESC_STRIDE = 128;
 constexpr int S1_LB_PER_LANE = 5;
 constexpr uint32_t DP_VALID = 1, DP_INCL = 2, DP_PAR = 4;
 constexpr uint32_t DA_VALID = 0x80000000u;
@@ -667,7 +645,7 @@ __device__ __forceinline__ uint32_t lookback_parity(uint8_t* dpar, int tile, uns
 #ifdef SJ_PROFILE_PHASES
             nspin++;
 #endif
-            if (SJ_SPIN_SLEEP && (again || SJ_SPIN_FIRST)) __nanosleep(SJ_SPIN_SLEEP);
+            if (again) __nanosleep(S1_SPIN_SLEEP_NS);
             again = true;
             ok = 1;
 #pragma unroll
@@ -714,7 +692,7 @@ __device__ __forceinline__ uint64_t lookback_count(uint8_t* dcnt, int tile, unsi
 #ifdef SJ_PROFILE_PHASES
             nspin++;
 #endif
-            if (SJ_SPIN_SLEEP && (again || SJ_SPIN_FIRST)) __nanosleep(SJ_SPIN_SLEEP);
+            if (again) __nanosleep(S1_SPIN_SLEEP_NS);
             again = true;
             ok = DA_VALID;
 #pragma unroll

@@ -31,48 +31,15 @@ constexpr int S2_TILE = S2_THREADS * S2_ITEMS;     // structurals per block = gr
 // Strings that need the byte-exact slow paths (escapes, or no escape-free proof from K1's backslash
 // map) are handled by their own thread up to this extent and by the whole warp beyond it: one long
 // string per warp would otherwise keep 31 lanes idle for hundreds of serial iterations.
-#ifndef SJ_S2_COOP_MIN
-#define SJ_S2_COOP_MIN 64
-#endif
-constexpr uint32_t S2_COOP_MIN = SJ_S2_COOP_MIN;  // 0xffffffff: never (thread-serial paths only)
-#ifndef SJ_S2_DENSE_NUMBERS
-#define SJ_S2_DENSE_NUMBERS 1
-#endif
-constexpr bool S2_DENSE_NUMBERS = SJ_S2_DENSE_NUMBERS != 0;  // number-heavy documents: numbers parsed by their own dense kernel
-// tuning knobs for variant builds (tools/build_variants.sh -> build_variants/*.so)
-#ifndef SJ_S2_DENSE_NUMBERS_SHIFT
-#define SJ_S2_DENSE_NUMBERS_SHIFT 4  // dense kernels when numbers << SHIFT >= structurals (one structural in 16)
-#endif
-#ifndef SJ_S2_EMIT_MIN_BLOCKS
-#define SJ_S2_EMIT_MIN_BLOCKS 8  // K2c: resident blocks per SM the register allocation must allow (8 = 32 registers)
-#endif
-#ifndef SJ_S2_NUMBERS_MIN_BLOCKS
-#define SJ_S2_NUMBERS_MIN_BLOCKS 0  // K2h: 0 = only the block size is given (ptxas settles at 32 registers + small spills today)
-#endif
-#ifndef SJ_S2_FAST_ESCAPES
-#define SJ_S2_FAST_ESCAPES 1
-#endif
-constexpr bool S2_FAST_ESCAPES = SJ_S2_FAST_ESCAPES != 0;  // warp routines decode all escapes of a window at once (warp_string_fast)
-// K2c (unescape): windows with one or two backslashes take the exact step instead of decoding every window.
-// K2a (measure): see SJ_S2_FAST_MEASURE.
-#ifndef SJ_S2_FAST_MIN_BACKSLASHES
-#define SJ_S2_FAST_MIN_BACKSLASHES 3
-#endif
-// K2a's long-string measure: 0 = exact warp routine, 1 = warp_string_fast inlined (the inlined routine changes the
-// code of the whole kernel), 2 = warp_string_fast behind a call
-#ifndef SJ_S2_FAST_MEASURE
-#define SJ_S2_FAST_MEASURE 2
-#endif
-
-
-// K2c short-string copy (the source line with 30 % of K2c's instructions): by default ptxas forms both 64-bit lane
-// addresses again under each of the four predicated steps (LDC.64 + IADD3 + IADD3.X twice: 9 instructions per step);
-// with 1 an empty asm pins the two bases in registers and the steps become ISETP + LDG + STG with immediate offsets.
-// Built and its SASS inspected, NOT yet run on a GPU (the round's GPU budget was spent): the default stays 0 until it
-// has passed the GPU suite -- first candidate of the next round (tools/build_variants.sh pinned="-DSJ_S2_COPY_PINNED_BASE=1").
-#ifndef SJ_S2_COPY_PINNED_BASE
-#define SJ_S2_COPY_PINNED_BASE 0
-#endif
+constexpr uint32_t S2_COOP_MIN = 64;
+// number-heavy documents get their numbers parsed by dense kernels (K2g / K2h) when numbers << SHIFT >= structurals
+// (one structural in 16)
+constexpr int S2_DENSE_NUMBERS_SHIFT = 4;
+constexpr int S2_EMIT_MIN_BLOCKS = 8;  // K2c: resident blocks per SM the register allocation must allow (8 = 32 registers)
+// Long strings with escapes: the warp routines decode all escapes of a window at once (warp_string_fast).  K2c
+// (unescape): windows with fewer backslashes than this take the exact step instead of decoding every window.  K2a
+// (measure) calls warp_string_fast behind a call (inlined, it changes the code of the whole kernel).
+constexpr int S2_FAST_MIN_BACKSLASHES = 3;
 
 struct ScanVal {
     uint32_t w;     // tape words
@@ -842,17 +809,11 @@ __global__ void __launch_bounds__(S2_THREADS) s2_classify_measure_kernel(const S
             const uint64_t ps = __shfl_sync(FULL, pos[j], owner), next_pos = __shfl_sync(FULL, nxt[j], owner);
             const StrCursor sc{p.msg + ps + 1, p.len - ps - 1};
             uint64_t sl = 0, dl = 0;
-            bool ok;
-            if (S2_FAST_ESCAPES && SJ_S2_FAST_MEASURE != 0) {
-                // the fast routine has no per-step bound test: its answer stands when the string closes inside the
-                // bound (every step of the exact routine then starts below it); anything else the exact one decides
-                const int r = SJ_S2_FAST_MEASURE == 2 ? warp_string_fast_measure_call(sc.body, sc.avail, next_pos - ps, &sl, &dl)
-                                                      : warp_string_fast<false, 1>(sc, next_pos - ps, nullptr, &sl, &dl);
-                ok = r == 1;
-                if (r == 2 || (r == 1 && sl >= next_pos - ps)) ok = warp_string_measure(sc, next_pos - ps, &sl, &dl);
-            } else {
-                ok = warp_string_measure(sc, next_pos - ps, &sl, &dl);
-            }
+            // the fast routine has no per-step bound test: its answer stands when the string closes inside the
+            // bound (every step of the exact routine then starts below it); anything else the exact one decides
+            const int r = warp_string_fast_measure_call(sc.body, sc.avail, next_pos - ps, &sl, &dl);
+            bool ok = r == 1;
+            if (r == 2 || (r == 1 && sl >= next_pos - ps)) ok = warp_string_measure(sc, next_pos - ps, &sl, &dl);
             if (ok && (int)(threadIdx.x & 31) == owner) {
                 typ4 |= (uint32_t)T_STRING << (8 * j);  // was T_INVALID
                 auxv[j] = (uint32_t)dl | ((p.copy_strings || sl != dl) ? AUX_COPY : 0) | (sl != dl ? AUX_ESC : 0);
@@ -947,7 +908,7 @@ __global__ void __launch_bounds__(1024) s2_scan_top_kernel(const ScanVal* in, ui
 // ---------------------------------------------------------------------------------
 // One structural per thread, warps independent of each other: with four structurals per thread the
 // tape stores of a warp spread over 32 sectors.
-__global__ void __launch_bounds__(S2_THREADS, SJ_S2_EMIT_MIN_BLOCKS) s2_emit_kernel(const Stage2Params p) {  // 8 blocks per SM = 32 registers: the kernel hides its load latency with occupancy
+__global__ void __launch_bounds__(S2_THREADS, S2_EMIT_MIN_BLOCKS) s2_emit_kernel(const Stage2Params p) {  // 8 blocks per SM = 32 registers: the kernel hides its load latency with occupancy
     const uint32_t i = blockIdx.x * S2_THREADS + threadIdx.x;
     const uint32_t lane = threadIdx.x & 31;
     uint32_t t = T_INVALID, aux = 0;
@@ -1051,18 +1012,9 @@ __global__ void __launch_bounds__(S2_THREADS, SJ_S2_EMIT_MIN_BLOCKS) s2_emit_ker
             const uint4 d = q[r];
             const uint8_t* src = p.msg + d.x;
             uint8_t* dst = p.strings + d.y;
-#if SJ_S2_COPY_PINNED_BASE
-            const uint8_t* sb = src + b;
-            uint8_t* db = dst + b;
-            asm volatile("" : "+l"(sb), "+l"(db));  // the lane bases stay in registers: [base + 8 k] in the four steps
-#pragma unroll
-            for (uint32_t o = 0; o < 32; o += 8)
-                if (o + b < d.z) db[o] = sb[o];
-#else
 #pragma unroll
             for (uint32_t o = 0; o < 32; o += 8)  // (a loop bounded by the length was measured: no difference)
                 if (o + b < d.z) dst[o + b] = src[o + b];
-#endif
         }
         uint32_t m = longm;
         while (m) {
@@ -1083,12 +1035,8 @@ __global__ void __launch_bounds__(S2_THREADS, SJ_S2_EMIT_MIN_BLOCKS) s2_emit_ker
         const uint64_t sp = __shfl_sync(FULL, (uint32_t)pos, owner);
         const uint32_t dp = __shfl_sync(FULL, e.str, owner);
         const StrCursor s{p.msg + sp + 1, p.len - sp - 1};
-        if (S2_FAST_ESCAPES) {
-            uint64_t sl_unused, dl_unused;
-            warp_string_fast<true, (int)SJ_S2_FAST_MIN_BACKSLASHES>(s, ~0ull, p.strings + dp, &sl_unused, &dl_unused);  // validated by K2a
-        } else {
-            warp_string_copy(s, p.strings + dp);
-        }
+        uint64_t sl_unused, dl_unused;
+        warp_string_fast<true, S2_FAST_MIN_BACKSLASHES>(s, ~0ull, p.strings + dp, &sl_unused, &dl_unused);  // validated by K2a
     }
 }
 
@@ -1125,11 +1073,7 @@ __global__ void __launch_bounds__(1024) s2_numlist_kernel(const Stage2Params p, 
     }
 }
 
-#if SJ_S2_NUMBERS_MIN_BLOCKS
-__global__ void __launch_bounds__(S2_THREADS, SJ_S2_NUMBERS_MIN_BLOCKS) s2_numbers_kernel(const Stage2Params p, uint32_t count) {
-#else
 __global__ void __launch_bounds__(S2_THREADS) s2_numbers_kernel(const Stage2Params p, uint32_t count) {
-#endif
     const uint32_t k = blockIdx.x * S2_THREADS + threadIdx.x;
     if (k >= count) return;
     const uint32_t i = p.numlist[k];

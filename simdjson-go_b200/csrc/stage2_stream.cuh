@@ -3,8 +3,8 @@
 //   K2p s2s_count      one warp per 6 KiB slab: per-slab aggregate (tape words, string bytes, brackets, depth, records,
 //                      structurals, numbers, bytes behind the last quote)
 //   K2q s2s_scan_*     exclusive scan of the aggregates (groups of 1024 + their totals), grand totals -> Stage2Result
-//   K2r s2s_emit       the same analysis again, now with every offset known: tape words and Strings.B bytes staged in
-//                      shared memory and streamed out with coalesced / 16-byte stores, bracket records for the scope
+//   K2r s2s_emit       the same analysis again, now with every offset known: tape words, Strings.B bytes (compacted in
+//                      shared memory and streamed out with coalesced / 16-byte stores), bracket records for the scope
 //                      matching, number list, per-segment grammar masks
 //   K2h s2s_numbers    parse_number (parse_number.go:65) over the number list, one number per thread
 //   K2d s2_min32 + s2_ansv (stage2.cuh)    scope matching on the brackets
@@ -28,23 +28,17 @@ namespace sj {
 static_assert(S2S_SLAB_BYTES == (uint32_t)S1_SLAB_BYTES, "stage 2 takes the in-string state per stage-1 slab");
 static_assert(S1_WARPS <= 32, "one bit per slab of a tile");
 
-#ifndef SJ_S2S_WARPS
-#define SJ_S2S_WARPS 8
-#endif
-constexpr int S2S_WARPS = SJ_S2S_WARPS;  // slabs per CTA
+constexpr int S2S_WARPS = 8;  // slabs per CTA
 constexpr int S2S_THREADS = S2S_WARPS * 32;
 constexpr uint32_t S2S_SSTAGE_PAD = (S2S_SSTAGE_BYTES + 15u) & ~15u;
 constexpr uint32_t S2S_WARP_SMEM_COUNT = S2S_IMAGE_BYTES + S2S_ESC_SCRATCH;
-static_assert(S2S_TSTAGE_WORDS * 8 >= S2S_ESC_SCRATCH, "K2r decodes escapes in the (then idle) tape staging area");
+static_assert(S2S_TSTAGE_WORDS * 8 >= S2S_ESC_SCRATCH, "K2r decodes escapes in the tape-staging area");
 constexpr uint32_t S2S_WARP_SMEM_EMIT = S2S_IMAGE_BYTES + S2S_SSTAGE_PAD + S2S_TSTAGE_WORDS * 8;
 constexpr size_t S2S_SMEM_COUNT = (size_t)S2S_WARPS * S2S_WARP_SMEM_COUNT;
 constexpr size_t S2S_SMEM_EMIT = (size_t)S2S_WARPS * S2S_WARP_SMEM_EMIT;
-#ifndef SJ_S2S_EMIT_MIN_BLOCKS
-#define SJ_S2S_EMIT_MIN_BLOCKS 2
-#endif
-#ifndef SJ_S2S_COUNT_MIN_BLOCKS
-#define SJ_S2S_COUNT_MIN_BLOCKS 3
-#endif
+// resident blocks per SM the register allocation must allow; also the persistent grids' blocks per SM
+constexpr int S2S_EMIT_MIN_BLOCKS = 2;
+constexpr int S2S_COUNT_MIN_BLOCKS = 3;
 
 struct DevWarp {
     __device__ __forceinline__ uint32_t lane() const { return threadIdx.x & 31; }
@@ -82,7 +76,7 @@ __device__ __forceinline__ void s2s_fill_tables(S2sTables& t) {
     if (threadIdx.x < 16) t.cmptab[threadIdx.x] = compress_sel(threadIdx.x) | ((uint32_t)__popc(threadIdx.x) << 16);
 }
 
-__global__ void __launch_bounds__(S2S_THREADS, SJ_S2S_COUNT_MIN_BLOCKS) s2s_count_kernel(const S2sParams p) {
+__global__ void __launch_bounds__(S2S_THREADS, S2S_COUNT_MIN_BLOCKS) s2s_count_kernel(const S2sParams p) {
     extern __shared__ __align__(128) uint8_t s2s_smem[];
     __shared__ S2sTables tabs;
     s2s_fill_tables(tabs);
@@ -100,7 +94,7 @@ __global__ void __launch_bounds__(S2S_THREADS, SJ_S2S_COUNT_MIN_BLOCKS) s2s_coun
     s2s_warp_loop<DevWarp, false>(wp, p, blockIdx.x * S2S_WARPS + warp, gridDim.x * S2S_WARPS, sm);
 }
 
-__global__ void __launch_bounds__(S2S_THREADS, SJ_S2S_EMIT_MIN_BLOCKS) s2s_emit_kernel(const S2sParams p) {
+__global__ void __launch_bounds__(S2S_THREADS, S2S_EMIT_MIN_BLOCKS) s2s_emit_kernel(const S2sParams p) {
     extern __shared__ __align__(128) uint8_t s2s_smem[];
     __shared__ S2sTables tabs;
     s2s_fill_tables(tabs);

@@ -8,7 +8,7 @@ import ctypes as C
 import os
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
-LIB_PATH = os.environ.get("SJ_B200_LIB") or os.path.join(os.path.dirname(_HERE), "libsimdjson_b200.so")  # override: kernel variants under test
+LIB_PATH = os.environ.get("SJ_B200_LIB") or os.path.join(os.path.dirname(_HERE), "libsimdjson_b200.so")  # override: another build, e.g. to compare two
 
 ERR_EXCHANGE, ERR_PEER, EXCHANGE_HANDLE_BYTES = 10, 11, 64
 FLAG_NDJSON = 1

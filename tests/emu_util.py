@@ -7,7 +7,7 @@ import numpy as np
 
 _DIR = os.path.join(os.path.dirname(os.path.abspath(__file__)), "emu")
 _SRC = os.path.join(_DIR, "s2s_emu.cpp")
-_FLAGS = os.environ.get("S2S_EMU_FLAGS", "").split()  # e.g. -DSJ_S2S_IMAGE_STEPS=1: the other shared-memory layout
+_FLAGS = os.environ.get("S2S_EMU_FLAGS", "").split()  # e.g. -DS2S_EMU_REVERSE: the lanes run in descending order
 _LIB = os.path.join(_DIR, "libs2semu%s.so" % ("_" + "_".join(f.strip("-").replace("=", "") for f in _FLAGS) if _FLAGS else ""))
 _CSRC = os.path.join(os.path.dirname(_DIR), "..", "simdjson-go_b200", "csrc")
 _lib = None
