@@ -21,16 +21,7 @@
 // This header is portable C++: under nvcc the functions are __host__ __device__, and tests/emu/s2s_emu.cpp compiles
 // the very same templates with a 32-fiber "warp" to check them against the oracle on a machine without a GPU.
 #pragma once
-#include <stdint.h>
-#include <stddef.h>
-
-#if defined(__CUDACC__)
-#define SJ_HD __host__ __device__ __forceinline__
-#define SJ_HDC __host__ __device__ constexpr
-#else
-#define SJ_HD inline
-#define SJ_HDC constexpr
-#endif
+#include "bits.h"
 
 namespace sj {
 
@@ -122,102 +113,11 @@ SJ_HDC uint32_t char_type(uint32_t ch) {
 
 constexpr uint64_t STRINGBUFBIT = 0x80000000000000ull;  // parsed_json.go:29
 
-// ---------------------------------------------------------------------------------
-// portable "intrinsics"
-// ---------------------------------------------------------------------------------
-namespace pi {
-SJ_HD uint32_t popc32(uint32_t x) {
-#ifdef __CUDA_ARCH__
-    return (uint32_t)__popc(x);
-#else
-    return (uint32_t)__builtin_popcount(x);
-#endif
-}
-SJ_HD uint32_t popc64(uint64_t x) {
-#ifdef __CUDA_ARCH__
-    return (uint32_t)__popcll(x);
-#else
-    return (uint32_t)__builtin_popcountll(x);
-#endif
-}
-SJ_HD uint32_t clz32(uint32_t x) {  // 32 for 0
-#ifdef __CUDA_ARCH__
-    return (uint32_t)__clz((int)x);
-#else
-    return x ? (uint32_t)__builtin_clz(x) : 32u;
-#endif
-}
-SJ_HD uint32_t clz64(uint64_t x) {  // 64 for 0
-#ifdef __CUDA_ARCH__
-    return (uint32_t)__clzll((long long)x);
-#else
-    return x ? (uint32_t)__builtin_clzll(x) : 64u;
-#endif
-}
-SJ_HD uint32_t ctz64(uint64_t x) {  // undefined for 0
-#ifdef __CUDA_ARCH__
-    return (uint32_t)__ffsll((long long)x) - 1u;
-#else
-    return (uint32_t)__builtin_ctzll(x);
-#endif
-}
-SJ_HD uint32_t ctz32(uint32_t x) {  // undefined for 0
-#ifdef __CUDA_ARCH__
-    return (uint32_t)__ffs((int)x) - 1u;
-#else
-    return (uint32_t)__builtin_ctz(x);
-#endif
-}
-SJ_HD uint32_t byte_perm(uint32_t a, uint32_t b, uint32_t sel) {  // selectors 0..7 only
-#ifdef __CUDA_ARCH__
-    return __byte_perm(a, b, sel);
-#else
-    const uint64_t pool = ((uint64_t)b << 32) | a;
-    uint32_t r = 0;
-    for (int i = 0; i < 4; i++) r |= (uint32_t)((pool >> (8 * ((sel >> (4 * i)) & 7))) & 0xff) << (8 * i);
-    return r;
-#endif
-}
-SJ_HD uint32_t shr_hi(uint32_t y, int s) {  // y >> s for 1 <= s <= 31, on the FMA pipe (IMAD.HI) on the device
-#ifdef __CUDA_ARCH__
-    return __umulhi(y, 1u << (32 - s));
-#else
-    return y >> s;
-#endif
-}
-SJ_HD uint32_t bitsel(uint32_t m, uint32_t a, uint32_t b) {  // (a & m) | (b & ~m), one LOP3
-#ifdef __CUDA_ARCH__
-    uint32_t d;
-    asm("lop3.b32 %0, %1, %2, %3, 0xE4;" : "=r"(d) : "r"(a), "r"(b), "r"(m));
-    return d;
-#else
-    return (a & m) | (b & ~m);
-#endif
-}
-SJ_HD uint32_t funnel_r(uint32_t lo, uint32_t hi, uint32_t s) {  // lower word of (hi:lo) >> (s & 31)
-#ifdef __CUDA_ARCH__
-    return __funnelshift_r(lo, hi, s);
-#else
-    s &= 31;
-    return s ? (lo >> s) | (hi << (32 - s)) : lo;
-#endif
-}
-SJ_HD uint32_t funnel_l(uint32_t lo, uint32_t hi, uint32_t s) {  // upper word of (hi:lo) << (s & 31)
-#ifdef __CUDA_ARCH__
-    return __funnelshift_l(lo, hi, s);
-#else
-    s &= 31;
-    return s ? (hi << s) | (lo >> (32 - s)) : hi;
-#endif
-}
-}  // namespace pi
-
 // 16 bytes moved as one vector access (LDS.128 / LDG.128 / STG.128 on the device)
 struct alignas(16) V16 {
     uint32_t x, y, z, w;
 };
 
-SJ_HD uint64_t mk64u(uint32_t lo, uint32_t hi) { return ((uint64_t)hi << 32) | lo; }
 SJ_HD uint64_t below64(uint32_t b) { return b >= 64 ? ~0ull : ((1ull << b) - 1ull); }  // bits [0, b)
 SJ_HD uint64_t lt64(uint32_t b) { return (1ull << b) - 1ull; }                         // bits [0, b), b < 64
 // the events of EV that follow an event of A (A a subset of EV; `cin`: the last event in front of the block is in A):
@@ -268,41 +168,10 @@ SJ_HD SlabAgg agg_combine(const SlabAgg& a, const SlabAgg& b) {
 }
 
 // ---------------------------------------------------------------------------------
-// byte classification: bit planes of 32 bytes, then every class as a Boolean function of the planes
-// (find_whitespace_and_structurals_amd64.s:6-29 and the compares of the other stage-1 routines; same scheme as
+// byte classification: bit planes of 32 bytes (bit_planes32, bits.h), then every class as a Boolean function of the
+// planes (find_whitespace_and_structurals_amd64.s:6-29 and the compares of the other stage-1 routines; same scheme as
 // stage1.cuh, with the classes stage 2 needs on top: brackets by direction, first bytes of numbers / atoms)
 // ---------------------------------------------------------------------------------
-SJ_HD void transpose4x4p(uint32_t a, uint32_t b, uint32_t c, uint32_t d, uint32_t& r0, uint32_t& r1, uint32_t& r2, uint32_t& r3) {
-    const uint32_t t0 = pi::byte_perm(a, b, 0x5140), t1 = pi::byte_perm(a, b, 0x7362);
-    const uint32_t t2 = pi::byte_perm(c, d, 0x5140), t3 = pi::byte_perm(c, d, 0x7362);
-    r0 = pi::byte_perm(t0, t2, 0x5410);
-    r1 = pi::byte_perm(t0, t2, 0x7632);
-    r2 = pi::byte_perm(t1, t3, 0x5410);
-    r3 = pi::byte_perm(t1, t3, 0x7632);
-}
-SJ_HD void s2p_pairp(uint32_t X, uint32_t Y, uint32_t m, int s, uint32_t& hi, uint32_t& lo) {
-    hi = pi::bitsel(m, X, pi::shr_hi(Y, s));
-    lo = pi::bitsel(m, X << s, Y);
-}
-// w[0..7]: 32 bytes (word k = bytes 4k..4k+3); pl[k] bit i = bit k of byte i
-SJ_HD void bit_planes32p(const uint32_t* w, uint32_t (&pl)[8]) {
-    uint32_t R[8];
-    transpose4x4p(w[0], w[2], w[4], w[6], R[0], R[1], R[2], R[3]);
-    transpose4x4p(w[1], w[3], w[5], w[7], R[4], R[5], R[6], R[7]);
-    uint32_t h1[4], l1[4];
-#pragma unroll
-    for (int t = 0; t < 4; t++) s2p_pairp(R[t + 4], R[t], 0xF0F0F0F0u, 4, h1[t], l1[t]);
-    uint32_t hh[2], hl[2], lh[2], ll[2];
-    s2p_pairp(h1[2], h1[0], 0xCCCCCCCCu, 2, hh[0], hl[0]);
-    s2p_pairp(h1[3], h1[1], 0xCCCCCCCCu, 2, hh[1], hl[1]);
-    s2p_pairp(l1[2], l1[0], 0xCCCCCCCCu, 2, lh[0], ll[0]);
-    s2p_pairp(l1[3], l1[1], 0xCCCCCCCCu, 2, lh[1], ll[1]);
-    s2p_pairp(hh[1], hh[0], 0xAAAAAAAAu, 1, pl[7], pl[6]);
-    s2p_pairp(hl[1], hl[0], 0xAAAAAAAAu, 1, pl[5], pl[4]);
-    s2p_pairp(lh[1], lh[0], 0xAAAAAAAAu, 1, pl[3], pl[2]);
-    s2p_pairp(ll[1], ll[0], 0xAAAAAAAAu, 1, pl[1], pl[0]);
-}
-
 struct Half2 {
     uint32_t bs, qt, ws, nl, open, close, cc, comma, curly, numc, atomc;
 };
@@ -342,39 +211,22 @@ struct Class64 {
 // w[16]: the block's 64 bytes in natural order
 SJ_HD Class64 classify_block2(const uint32_t (&w)[16]) {
     uint32_t p0[8], p1[8];
-    bit_planes32p(&w[0], p0);
-    bit_planes32p(&w[8], p1);
+    bit_planes32(&w[0], p0);
+    bit_planes32(&w[8], p1);
     const Half2 a = classify_planes2(p0), b = classify_planes2(p1);
     Class64 m;
-    m.bs = mk64u(a.bs, b.bs);
-    m.qt = mk64u(a.qt, b.qt);
-    m.ws = mk64u(a.ws, b.ws);
-    m.nl = mk64u(a.nl, b.nl);
-    m.open = mk64u(a.open, b.open);
-    m.close = mk64u(a.close, b.close);
-    m.cc = mk64u(a.cc, b.cc);
-    m.comma = mk64u(a.comma, b.comma);
-    m.curly = mk64u(a.curly, b.curly);
-    m.numc = mk64u(a.numc, b.numc);
-    m.atomc = mk64u(a.atomc, b.atomc);
+    m.bs = mk64(a.bs, b.bs);
+    m.qt = mk64(a.qt, b.qt);
+    m.ws = mk64(a.ws, b.ws);
+    m.nl = mk64(a.nl, b.nl);
+    m.open = mk64(a.open, b.open);
+    m.close = mk64(a.close, b.close);
+    m.cc = mk64(a.cc, b.cc);
+    m.comma = mk64(a.comma, b.comma);
+    m.curly = mk64(a.curly, b.curly);
+    m.numc = mk64(a.numc, b.numc);
+    m.atomc = mk64(a.atomc, b.atomc);
     return m;
-}
-
-// find_quote_mask_and_bits_amd64.s:66: carry-less multiply by all-ones == prefix XOR
-SJ_HD uint64_t prefix_xor64p(uint64_t x) {
-    uint32_t lo = (uint32_t)x, hi = (uint32_t)(x >> 32);
-    lo ^= lo << 1;
-    hi ^= hi << 1;
-    lo ^= lo << 2;
-    hi ^= hi << 2;
-    lo ^= lo << 4;
-    hi ^= hi << 4;
-    lo ^= lo << 8;
-    hi ^= hi << 8;
-    lo ^= lo << 16;
-    hi ^= hi << 16;
-    hi ^= (uint32_t)((int32_t)lo >> 31);
-    return mk64u(lo, hi);
 }
 
 // Escape STARTS of a block: the backslashes that sit at an even offset inside their run (every second one, beginning
@@ -392,27 +244,6 @@ SJ_HD uint64_t escape_starts(uint64_t bs, uint32_t first_escaped) {
 // ---------------------------------------------------------------------------------
 // escapes (parse_string_amd64.s:101-229; accept / reject behaviour as restated in stage2.cuh escape_step)
 // ---------------------------------------------------------------------------------
-SJ_HD int32_t digit_to_val_p(uint32_t c) {  // parse_string_amd64.s:4-69: bytes below '0' read as 0
-    if (c < 0x30) return 0;
-    if (c <= '9') return (int32_t)c - '0';
-    const uint32_t l = c | 0x20;
-    if (c < 0x80 && l >= 'a' && l <= 'f' && c >= 'A') return (int32_t)l - 'a' + 10;
-    return -1;
-}
-SJ_HD uint32_t escape_map_p(uint32_t e) {
-    switch (e) {
-    case '"': return 0x22;
-    case '/': return 0x2f;
-    case '\\': return 0x5c;
-    case 'b': return 0x08;
-    case 'f': return 0x0c;
-    case 'n': return 0x0a;
-    case 'r': return 0x0d;
-    case 't': return 0x09;
-    default: return 0;
-    }
-}
-
 struct EscInfo {
     uint32_t c;      // source bytes consumed (2, 6 or 12); 0 for the second half of a surrogate pair
     uint32_t n;      // UTF-8 bytes produced (1..4)
@@ -427,8 +258,8 @@ template <class R>
 SJ_HD uint32_t hex4_at(const R& rd, uint64_t x) {
     const uint32_t c0 = rd(x), c1 = rd(x + 1), c2 = rd(x + 2), c3 = rd(x + 3);
     if (c0 == '"' || c1 == '"' || c2 == '"' || c3 == '"') return 0xffffffffu;
-    const uint32_t v = ((uint32_t)digit_to_val_p(c0) << 12) | ((uint32_t)digit_to_val_p(c1) << 8) | ((uint32_t)digit_to_val_p(c2) << 4) |
-                       (uint32_t)digit_to_val_p(c3);
+    const uint32_t v = ((uint32_t)digit_to_val(c0) << 12) | ((uint32_t)digit_to_val(c1) << 8) | ((uint32_t)digit_to_val(c2) << 4) |
+                       (uint32_t)digit_to_val(c3);
     return v > 0xffffu ? 0xffffffffu : v;
 }
 // number of consecutive backslashes immediately in front of x
@@ -453,13 +284,6 @@ SJ_HD bool high_escape_at(const N& near, const F& far, uint64_t y) {
     return (backslashes_before(far, y) & 1u) == 0;
 }
 
-SJ_HD uint32_t utf8_pack(uint32_t cp, uint32_t n) {
-    if (n == 1) return cp;
-    if (n == 2) return (0xC0u + (cp >> 6)) | ((0x80u | (cp & 63)) << 8);
-    if (n == 3) return (0xE0u + (cp >> 12)) | ((0x80u | ((cp >> 6) & 63)) << 8) | ((0x80u | (cp & 63)) << 16);
-    return (0xF0u + (cp >> 18)) | ((0x80u | ((cp >> 12) & 63)) << 8) | ((0x80u | ((cp >> 6) & 63)) << 16) | ((0x80u | (cp & 63)) << 24);
-}
-
 // the escape whose backslash sits at x (x is known to be an escape start).  rd(pos) returns the ORIGINAL message
 // byte, 0 beyond its end.  The sequential decoder consumes a surrogate pair in one step; here the "\u" of the low
 // half is an escape start of its own, recognised by walking the chain of high surrogates in front of it: it is a
@@ -473,7 +297,7 @@ SJ_HD EscInfo esc_decode(const R& rd, const B& far, uint64_t x) {
     r.c = 2, r.n = 1, r.bytes = 0, r.valid = true, r.second = false;
     const uint32_t e = rd(x + 1);
     if (e != 'u') {
-        const uint32_t m = escape_map_p(e);
+        const uint32_t m = escape_map(e);
         r.valid = m != 0;
         r.bytes = m;
         return r;

@@ -47,10 +47,6 @@ struct GlobalReader {
 };
 
 // atoms (stage2_build_tape_amd64.go:124-158, 455-476): literal + one following byte that is structural / white / NUL
-SJ_HD bool structural_or_ws_or_nul_p(uint32_t c) {
-    return c == 0 || c == '\t' || c == '\n' || c == '\r' || c == ' ' || c == ',' || c == ':' || c == '[' || c == ']' ||
-           c == '{' || c == '}';
-}
 template <class R>
 SJ_HD bool atom_ok_p(const R& rd, uint64_t pos, uint64_t len, uint32_t type) {
     const char* lit = type == T_TRUE ? "true" : type == T_FALSE ? "false" : "null";
@@ -58,7 +54,7 @@ SJ_HD bool atom_ok_p(const R& rd, uint64_t pos, uint64_t len, uint32_t type) {
     if (pos + n + 1 > len) return false;  // len(buf) >= n + 1
     for (uint32_t i = 0; i < n; i++)
         if (rd(pos + i) != (uint32_t)(uint8_t)lit[i]) return false;
-    return structural_or_ws_or_nul_p(rd(pos + n));
+    return structural_or_ws_or_nul(rd(pos + n));
 }
 
 // The same test for an atom that lies, with the byte behind it and then some, inside the step image (o + 8 <= avail):
@@ -84,7 +80,7 @@ SJ_HD bool atom_ok_fast(const uint8_t* img, uint32_t o, uint32_t avail, uint32_t
     } else {
         return false;
     }
-    // NUL \t \n \r | space , : | [ ] | { }   (structural_or_ws_or_nul_p)
+    // NUL \t \n \r | space , : | [ ] | { }   (structural_or_ws_or_nul)
     const uint32_t set = follow < 32 ? 0x00002601u : follow < 64 ? 0x04001001u : follow < 96 ? 0x28000000u : 0x28000000u;
     *ok = lit && follow < 128 && ((set >> (follow & 31u)) & 1u) != 0;
     return true;
@@ -367,7 +363,7 @@ SJ_HD void s2s_slab(W& wp, const S2sParams& p, uint32_t slab, const S2sWarpMem& 
         {
             const uint32_t P = wp.ballot((pi::popc64(qb) & 1u) != 0);
             const uint32_t lane_in = par ^ (pi::popc32(P & lt) & 1u);
-            qm = prefix_xor64p(qb) ^ (lane_in ? ~0ull : 0ull);
+            qm = prefix_xor64(qb) ^ (lane_in ? ~0ull : 0ull);
             par ^= pi::popc32(P) & 1u;
         }
 
@@ -469,7 +465,7 @@ SJ_HD void s2s_slab(W& wp, const S2sParams& p, uint32_t slab, const S2sWarpMem& 
                 if (EMIT) wp.sync();
             }
             wp.sync();
-            D = mk64u(dmap[2 * lane], dmap[2 * lane + 1]);
+            D = mk64(dmap[2 * lane], dmap[2 * lane + 1]);
             hd_next.drop = dmap[S2S_ESC_DMAP_WORDS - 1];
             hd_next.nhead = rec[0], hd_next.hpos = rec[1], hd_next.head = rec[2];
             wp.sync();  // (the scratch is the tape staging area of the rest of the step)
@@ -569,7 +565,7 @@ SJ_HD void s2s_slab(W& wp, const S2sParams& p, uint32_t slab, const S2sWarpMem& 
                 const uint32_t tl = wp.shfl_up((uint32_t)inc, d), th = wp.shfl_up((uint32_t)(inc >> 32), d);
                 const uint32_t tn = wp.shfl_up(ninc, d);
                 if ((int)lane >= d) {
-                    inc += mk64u(tl, th);
+                    inc += mk64(tl, th);
                     ninc += tn;
                 }
             }
@@ -578,7 +574,7 @@ SJ_HD void s2s_slab(W& wp, const S2sParams& p, uint32_t slab, const S2sWarpMem& 
             r_ex = (uint32_t)((ex >> 37) & 0x7ff);
             d_ex = (int32_t)(ex >> 48) - 64 * (int32_t)lane;
             n_ex = ninc - n_num;
-            const uint64_t tot = mk64u(wp.shfl((uint32_t)inc, 31), wp.shfl((uint32_t)(inc >> 32), 31));
+            const uint64_t tot = mk64(wp.shfl((uint32_t)inc, 31), wp.shfl((uint32_t)(inc >> 32), 31));
             w_step = (uint32_t)(tot & 0x1fff), k_step = (uint32_t)((tot >> 13) & 0xfff), b_step = (uint32_t)((tot >> 25) & 0xfff);
             r_step = (uint32_t)((tot >> 37) & 0x7ff);
             d_step = (int32_t)(tot >> 48) - 64 * 32;

@@ -23,6 +23,7 @@
 // one tile ahead).  The 64-byte masks come from a bit-sliced classifier (byte transpose + bit
 // planes + Boolean class functions) instead of per-byte compares.
 #pragma once
+#include "bits.h"
 #include "common.cuh"
 #include "s2s_core.h"
 
@@ -104,8 +105,6 @@ __device__ __forceinline__ WordFlagsSlow classify_word_slow(uint32_t v) {
 __device__ __forceinline__ uint32_t gather4(uint32_t flags, uint32_t acc) {
     return __funnelshift_l(flags * 0x00204081u, acc, 4);
 }
-
-__device__ __forceinline__ uint64_t mk64(uint32_t lo, uint32_t hi) { return ((uint64_t)hi << 32) | lo; }
 
 // rotate a 64-bit mask left by 16*r bits (r = 0..3): undoes the bank-conflict-free
 // chunk rotation used when a lane reads its 64 bytes from shared memory
@@ -200,10 +199,12 @@ __device__ __forceinline__ SlowMasks classify_block_slow(const uint32_t (&w)[16]
 
 // ---------------------------------------------------------------------------------
 // Bit-sliced classification (default).  The 64 bytes of a block are transposed into their 8
-// bit planes (a 4x4 byte transpose with PRMT, then three mask/shift merge stages -- the
-// classic "s2p" of parallel bit streams), after which every class is a Boolean function of
-// the planes evaluated for 32 bytes per LOP3: no per-class compares, no flag gathering, and
-// tab / LF / CR / control masks come for free.  About 230 instructions per 64-byte block for
+// bit planes (bit_planes32 of bits.h, the same code the streaming stage 2 runs: a 4x4 byte
+// transpose with PRMT, then three mask/shift merge stages -- the classic "s2p" of parallel
+// bit streams), after which every class is a Boolean function of the planes evaluated for
+// 32 bytes per LOP3: no per-class compares, no flag gathering, and tab / LF / CR / control
+// masks come for free.  K1's class set differs from the streaming pass's (classify_planes2),
+// so the Boolean functions stay apart.  About 230 instructions per 64-byte block for
 // all six masks, against 464 (4 masks) to 750 (with the control-character pass) for the
 // word-wise SWAR compares above; those stay as an independent second implementation that the
 // test hook sj_test_block_masks cross-checks against this one on every block.
@@ -211,52 +212,6 @@ __device__ __forceinline__ SlowMasks classify_block_slow(const uint32_t (&w)[16]
 struct PlaneMasks {
     uint64_t bs, qt, st, ws, ct, nl;
 };
-
-// rows a,b,c,d (4 bytes each) -> r_t = {a.b_t, b.b_t, c.b_t, d.b_t}
-__device__ __forceinline__ void transpose4x4(uint32_t a, uint32_t b, uint32_t c, uint32_t d, uint32_t& r0, uint32_t& r1,
-                                             uint32_t& r2, uint32_t& r3) {
-    uint32_t t0 = __byte_perm(a, b, 0x5140), t1 = __byte_perm(a, b, 0x7362);
-    uint32_t t2 = __byte_perm(c, d, 0x5140), t3 = __byte_perm(c, d, 0x7362);
-    r0 = __byte_perm(t0, t2, 0x5410);
-    r1 = __byte_perm(t0, t2, 0x7632);
-    r2 = __byte_perm(t1, t3, 0x5410);
-    r3 = __byte_perm(t1, t3, 0x7632);
-}
-
-// one merge step: hi keeps the m-bits of X in place and moves the m-bits of Y down by s;
-// lo moves the ~m-bits of X up by s and keeps the ~m-bits of Y     (m >> s == ~m)
-// (a & m) | (b & ~m) as ONE LOP3 (the compiler emits an AND and an OR-AND for the C expression
-// because m and ~m are different immediates)
-__device__ __forceinline__ uint32_t bitsel(uint32_t m, uint32_t a, uint32_t b) {
-    uint32_t d;
-    asm("lop3.b32 %0, %1, %2, %3, 0xE4;" : "=r"(d) : "r"(a), "r"(b), "r"(m));
-    return d;
-}
-__device__ __forceinline__ void s2p_pair(uint32_t X, uint32_t Y, uint32_t m, int s, uint32_t& hi, uint32_t& lo) {
-    // Y >> s as IMAD.HI: the classifier is bound by the ALU pipe (LOP3 / SHF / PRMT issue every
-    // other cycle), the FMA pipe is nearly idle
-    hi = bitsel(m, X, __umulhi(Y, 1u << (32 - s)));
-    lo = bitsel(m, X << s, Y);
-}
-
-// bit planes of 32 bytes held in 8 words (word k = bytes 4k..4k+3): pl[k] bit i = bit k of byte i
-__device__ __forceinline__ void bit_planes32(const uint32_t* w, uint32_t (&pl)[8]) {
-    uint32_t R[8];  // R[t] = bytes {t, 8+t, 16+t, 24+t}
-    transpose4x4(w[0], w[2], w[4], w[6], R[0], R[1], R[2], R[3]);
-    transpose4x4(w[1], w[3], w[5], w[7], R[4], R[5], R[6], R[7]);
-    uint32_t h1[4], l1[4];
-#pragma unroll
-    for (int t = 0; t < 4; t++) s2p_pair(R[t + 4], R[t], 0xF0F0F0F0u, 4, h1[t], l1[t]);
-    uint32_t hh[2], hl[2], lh[2], ll[2];
-    s2p_pair(h1[2], h1[0], 0xCCCCCCCCu, 2, hh[0], hl[0]);
-    s2p_pair(h1[3], h1[1], 0xCCCCCCCCu, 2, hh[1], hl[1]);
-    s2p_pair(l1[2], l1[0], 0xCCCCCCCCu, 2, lh[0], ll[0]);
-    s2p_pair(l1[3], l1[1], 0xCCCCCCCCu, 2, lh[1], ll[1]);
-    s2p_pair(hh[1], hh[0], 0xAAAAAAAAu, 1, pl[7], pl[6]);
-    s2p_pair(hl[1], hl[0], 0xAAAAAAAAu, 1, pl[5], pl[4]);
-    s2p_pair(lh[1], lh[0], 0xAAAAAAAAu, 1, pl[3], pl[2]);
-    s2p_pair(ll[1], ll[0], 0xAAAAAAAAu, 1, pl[1], pl[0]);
-}
 
 struct HalfMasks {
     uint32_t bs, qt, st, ws, ct, nl;
@@ -317,23 +272,6 @@ __device__ __forceinline__ uint64_t odd_backslash_ends(uint64_t bs, uint32_t pre
     if (carry_out) *carry_out = odd_carries < bs;
     odd_carries |= p;
     return (even_carries & ~bs & odd_bits) | (odd_carries & ~bs & even_bits);
-}
-
-// find_quote_mask_and_bits_amd64.s:66: carry-less multiply by all-ones == prefix XOR
-__device__ __forceinline__ uint64_t prefix_xor64(uint64_t x) {
-    uint32_t lo = (uint32_t)x, hi = (uint32_t)(x >> 32);
-    lo ^= lo << 1;
-    hi ^= hi << 1;
-    lo ^= lo << 2;
-    hi ^= hi << 2;
-    lo ^= lo << 4;
-    hi ^= hi << 4;
-    lo ^= lo << 8;
-    hi ^= hi << 8;
-    lo ^= lo << 16;
-    hi ^= hi << 16;
-    hi ^= (uint32_t)((int32_t)lo >> 31);  // parity of the low half carries into the high half
-    return mk64(lo, hi);
 }
 
 // finalize_structurals_amd64.s:19-36 ; pp_in in {0,1}; *pp_out = pseudo_pred >> 63
@@ -730,7 +668,8 @@ __device__ __forceinline__ uint64_t lookback_count(uint8_t* dcnt, int tile, unsi
 
 // ---------------------------------------------------------------------------------
 // carries recovered from the bytes in front of a slab: length of the run of backslashes
-// that ends just before `end` (warp-cooperative, 32 bytes per round; one round in practice)
+// that ends just before `end` (warp-cooperative, 32 bytes per round; one round in practice).
+// Not backslash_run_before_p (s2s_slab.h): that one compiles to other bit-scan instructions.
 // ---------------------------------------------------------------------------------
 __device__ __forceinline__ uint32_t backslash_run_before(const uint8_t* __restrict__ msg, uint64_t end) {
     const uint32_t lane = threadIdx.x & 31;

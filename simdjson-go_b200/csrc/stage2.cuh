@@ -15,13 +15,16 @@
 //                         (previous two structurals, enclosing container); cross-links { } [ ]
 //   K2f roots             root words and NDJSON root chaining (stage2...go:190-221, 428-441)
 #pragma once
+#include <type_traits>
+
 #include "common.cuh"
 #include "number.cuh"
 #include "s2s_core.h"
 
 namespace sj {
 
-// structural types, the grammar (transition_ok) and STRINGBUFBIT live in s2s_core.h (shared with the streaming kernels)
+// structural types, the grammar (transition_ok) and STRINGBUFBIT live in s2s_core.h, the atom and escape tables
+// (structural_or_ws_or_nul, digit_to_val, escape_map) in bits.h: both are shared with the streaming kernels
 constexpr uint32_t AUX_COPY = 0x80000000u;              // string goes to the string buffer
 constexpr uint32_t AUX_ESC = 0x40000000u;               // string contains escapes (source length != unescaped length)
 constexpr uint32_t AUX_LEN = 0x3fffffffu;
@@ -49,7 +52,8 @@ struct ScanVal {
     int32_t depth;  // +1 open, -1 close
 };
 
-__device__ __forceinline__ ScanVal sv_add(const ScanVal& a, const ScanVal& b) {
+// agg_combine / agg_shfl_up: the operations of SlabAgg (s2s_core.h) for ScanVal, so that one block scan serves both
+__device__ __forceinline__ ScanVal agg_combine(const ScanVal& a, const ScanVal& b) {
     ScanVal r;
     r.w = a.w + b.w;
     r.brk = a.brk + b.brk;
@@ -59,7 +63,7 @@ __device__ __forceinline__ ScanVal sv_add(const ScanVal& a, const ScanVal& b) {
     return r;
 }
 __device__ __forceinline__ ScanVal sv_zero() { return ScanVal{0, 0, 0, 0, 0}; }
-__device__ __forceinline__ ScanVal sv_shfl_up(const ScanVal& a, int d) {
+__device__ __forceinline__ ScanVal agg_shfl_up(const ScanVal& a, int d) {
     ScanVal r;
     r.w = __shfl_up_sync(FULL, a.w, d);
     r.brk = __shfl_up_sync(FULL, a.brk, d);
@@ -68,50 +72,51 @@ __device__ __forceinline__ ScanVal sv_shfl_up(const ScanVal& a, int d) {
     r.depth = __shfl_up_sync(FULL, a.depth, d);
     return r;
 }
-__device__ __forceinline__ ScanVal sv_shfl(const ScanVal& a, int src) {
-    ScanVal r;
-    r.w = __shfl_sync(FULL, a.w, src);
-    r.brk = __shfl_sync(FULL, a.brk, src);
-    r.str = __shfl_sync(FULL, a.str, src);
-    r.rec = __shfl_sync(FULL, a.rec, src);
-    r.depth = __shfl_sync(FULL, a.depth, src);
+__device__ __forceinline__ SlabAgg agg_shfl_up(const SlabAgg& a, int d) {
+    SlabAgg r;
+    r.w = __shfl_up_sync(FULL, a.w, d);
+    r.str = __shfl_up_sync(FULL, a.str, d);
+    r.brk = __shfl_up_sync(FULL, a.brk, d);
+    r.rec = __shfl_up_sync(FULL, a.rec, d);
+    r.depth = __shfl_up_sync(FULL, a.depth, d);
+    r.ns = __shfl_up_sync(FULL, a.ns, d);
+    r.num = __shfl_up_sync(FULL, a.num, d);
+    r.trail = __shfl_up_sync(FULL, a.trail, d);
     return r;
 }
 
-// block-wide exclusive scan (blockDim.x = NT, a multiple of 32, <= 1024); returns the
-// exclusive prefix of the calling thread and the block total.  Warp totals are scanned by the
-// first warp so every thread reads just two entries of shared memory.
-template <int NT>
-__device__ __forceinline__ ScanVal block_exclusive_scan(ScanVal v, ScanVal& total) {
-    constexpr int NW = NT / 32;
-    __shared__ ScanVal warp_pre[NW + 1];  // [w] = sum of warps < w, [NW] = block total
+// block-wide exclusive scan of ScanVal (K2b) or SlabAgg (K2q), blockDim.x = 1024; returns the exclusive prefix of the
+// calling thread and the block total.  agg_combine(a, b) puts a in front of b (SlabAgg's is not commutative in
+// `trail`).  Warp totals are scanned by the first warp so every thread reads just two entries of shared memory.
+template <class T>
+__device__ __forceinline__ T block_exclusive_scan(const T& v, T& total) {
+    __shared__ T warp_inc[33];  // [w] = sum of warps < w, [32] = block total
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-    ScanVal inc = v;
+    T inc = v;
 #pragma unroll
     for (int d = 1; d < 32; d <<= 1) {
-        ScanVal t = sv_shfl_up(inc, d);
-        if (lane >= d) inc = sv_add(inc, t);
+        const T t = agg_shfl_up(inc, d);
+        if (lane >= d) inc = agg_combine(t, inc);
     }
-    if (lane == 31) warp_pre[warp + 1] = inc;  // provisional: the warp's own total
+    if (lane == 31) warp_inc[warp + 1] = inc;  // provisional: the warp's own total
     __syncthreads();
     if (warp == 0) {
-        ScanVal w = lane < NW ? warp_pre[lane + 1] : sv_zero();
+        T wv = warp_inc[lane + 1];
 #pragma unroll
-        for (int d = 1; d < NW; d <<= 1) {
-            ScanVal t = sv_shfl_up(w, d);
-            if (lane >= d) w = sv_add(w, t);
+        for (int d = 1; d < 32; d <<= 1) {
+            const T t = agg_shfl_up(wv, d);
+            if (lane >= d) wv = agg_combine(t, wv);
         }
         __syncwarp();
-        if (lane < NW) warp_pre[lane + 1] = w;  // inclusive: sum of warps <= lane
-        if (lane == 0) warp_pre[0] = sv_zero();
+        warp_inc[lane + 1] = wv;  // inclusive over warps <= lane
+        if (lane == 0) warp_inc[0] = T{};
     }
     __syncthreads();
-    total = warp_pre[NW];
-    ScanVal wpre = warp_pre[warp];
-    ScanVal exc = sv_shfl_up(inc, 1);
-    if (lane == 0) exc = sv_zero();
-    ScanVal r = sv_add(wpre, exc);
-    __syncthreads();  // the shared array may be reused by the next call
+    total = warp_inc[32];
+    T ex = agg_shfl_up(inc, 1);
+    if (lane == 0) ex = T{};
+    const T r = agg_combine(warp_inc[warp], ex);
+    __syncthreads();  // the shared array is reused by the next call
     return r;
 }
 
@@ -265,10 +270,6 @@ __device__ __forceinline__ uint64_t s2_str_base(const Stage2Params& p) { return 
 // ---------------------------------------------------------------------------------
 // atoms (stage2_build_tape_amd64.go:124-158, 455-476)
 // ---------------------------------------------------------------------------------
-__device__ __forceinline__ bool structural_or_ws_or_nul(uint32_t c) {
-    return c == 0 || c == '\t' || c == '\n' || c == '\r' || c == ' ' || c == ',' || c == ':' || c == '[' ||
-           c == ']' || c == '{' || c == '}';
-}
 __device__ __forceinline__ bool atom_ok(const uint8_t* m, uint64_t pos, uint64_t len, const char* lit, int n) {
     if (pos + n + 1 > len) return false;  // needs one byte after the literal (len(buf) >= n+1)
     for (int i = 0; i < n; i++)
@@ -279,29 +280,6 @@ __device__ __forceinline__ bool atom_ok(const uint8_t* m, uint64_t pos, uint64_t
 // ---------------------------------------------------------------------------------
 // strings
 // ---------------------------------------------------------------------------------
-// parse_string_amd64.s:4-69 digittoval: bytes below '0' map to 0 (no DATA line), hex digits to
-// their value, everything else to -1
-__device__ __forceinline__ int32_t digit_to_val(uint32_t c) {
-    if (c < 0x30) return 0;
-    if (c <= '9') return (int32_t)c - '0';
-    uint32_t l = c | 0x20;
-    if (c < 0x80 && l >= 'a' && l <= 'f' && c >= 'A') return (int32_t)l - 'a' + 10;
-    return -1;
-}
-__device__ __forceinline__ uint32_t escape_map(uint32_t e) {
-    switch (e) {
-    case '"': return 0x22;
-    case '/': return 0x2f;
-    case '\\': return 0x5c;
-    case 'b': return 0x08;
-    case 'f': return 0x0c;
-    case 'n': return 0x0a;
-    case 'r': return 0x0d;
-    case 't': return 0x09;
-    default: return 0;
-    }
-}
-
 struct StrCursor {
     const uint8_t* body;  // first byte after the opening quote
     uint64_t avail;       // bytes readable from body; beyond that the reference reads zeros
@@ -386,7 +364,8 @@ __device__ __forceinline__ bool string_measure(const StrCursor& s, uint64_t max_
     }
 }
 
-// _parse_string (parse_string_amd64.s:260-479) for a string that already validated
+// _parse_string (parse_string_amd64.s:260-479) for a string that already validated.  The UTF-8 bytes of an escape are
+// stored one by one here and in the warp routines below: packing them with utf8_pack (bits.h) changes those stores.
 __device__ __forceinline__ void string_copy(const StrCursor& s, uint8_t* dst) {
     uint64_t p = 0, dl = 0;
     for (;;) {
@@ -827,7 +806,7 @@ __global__ void __launch_bounds__(S2_THREADS) s2_classify_measure_kernel(const S
         if (i < p.n) {
             uint32_t next_t = T_START;  // only "newline or not" matters
             if (i + 1 < p.n) next_t = (j + 1 < S2_ITEMS ? c[(j + 1) & 3] : cn) == '\n' ? T_NEWLINE : T_INVALID;
-            v = sv_add(v, contribution((typ4 >> (8 * j)) & 0xff, auxv[j], next_t));
+            v = agg_combine(v, contribution((typ4 >> (8 * j)) & 0xff, auxv[j], next_t));
         }
     }
     if (i0 + S2_ITEMS <= p.n) {
@@ -864,29 +843,31 @@ __global__ void __launch_bounds__(S2_THREADS) s2_classify_measure_kernel(const S
 }
 
 // ---------------------------------------------------------------------------------
-// K2b: exclusive scan of `in[0..n)` in groups of 1024 (one block per group)
+// K2b (ScanVal per tile) / K2q (SlabAgg per slab): exclusive scan of `in[0..n)` in groups of 1024 (one block per group)
 // ---------------------------------------------------------------------------------
-__global__ void __launch_bounds__(1024) s2_scan_groups_kernel(const ScanVal* in, uint32_t n, ScanVal* pre,
-                                                              ScanVal* group_total) {
+template <class T>
+__global__ void __launch_bounds__(1024) scan_groups_kernel(const T* in, uint32_t n, T* pre, T* group_total) {
     const uint32_t i = blockIdx.x * 1024 + threadIdx.x;
-    ScanVal v = i < n ? in[i] : sv_zero();
-    ScanVal total;
-    ScanVal e = block_exclusive_scan<1024>(v, total);
+    const T v = i < n ? in[i] : T{};
+    T total;
+    const T e = block_exclusive_scan(v, total);
     if (i < n) pre[i] = e;
     if (threadIdx.x == 0) group_total[blockIdx.x] = total;
 }
 
-// single block: exclusive scan of all group totals (looping), grand total into result
-__global__ void __launch_bounds__(1024) s2_scan_top_kernel(const ScanVal* in, uint32_t n, ScanVal* pre,
-                                                           Stage2Result* res, uint64_t* totals_out, uint64_t msg_bytes) {
-    ScanVal carry = sv_zero();
+// single block: exclusive scan of all group totals (looping), grand totals into `res` and, when given, into
+// `totals_out` (sj_shard_totals in device memory, for an exchange that stays on the stream)
+template <class T>
+__global__ void __launch_bounds__(1024) scan_top_kernel(const T* in, uint32_t n, T* pre, Stage2Result* res, uint64_t* totals_out,
+                                                        uint64_t msg_bytes) {
+    T carry{};
     for (uint32_t base = 0; base < n; base += 1024) {
         const uint32_t i = base + threadIdx.x;
-        ScanVal v = i < n ? in[i] : sv_zero();
-        ScanVal total;
-        ScanVal e = block_exclusive_scan<1024>(v, total);
-        if (i < n) pre[i] = sv_add(carry, e);
-        carry = sv_add(carry, total);
+        const T v = i < n ? in[i] : T{};
+        T total;
+        const T e = block_exclusive_scan(v, total);
+        if (i < n) pre[i] = agg_combine(carry, e);
+        carry = agg_combine(carry, total);
     }
     if (threadIdx.x == 0) {
         res->tape_len = (uint64_t)carry.w + 2;  // + root open + root close
@@ -894,6 +875,7 @@ __global__ void __launch_bounds__(1024) s2_scan_top_kernel(const ScanVal* in, ui
         res->n_brackets = carry.brk;
         res->n_records = carry.rec;
         res->final_depth = carry.depth;
+        if constexpr (std::is_same<T, SlabAgg>::value) res->n_numbers = carry.num;  // (K2a adds up its own count)
         if (totals_out) {
             totals_out[0] = msg_bytes;
             totals_out[1] = (uint64_t)carry.w + 2;
@@ -925,8 +907,8 @@ __global__ void __launch_bounds__(S2_THREADS, S2_EMIT_MIN_BLOCKS) s2_emit_kernel
     // prefix in front of the warp's 32 structurals: K2b's tile prefix + K2a's prefix inside the tile;
     // the rest is a warp scan -- no shared memory, no barrier in this kernel
     const uint32_t tile = i / S2_TILE;
-    const ScanVal blk = sv_add(p.sub_pre[i >> 5], sv_add(p.tile_pre[tile], p.grp_pre[tile >> 10]));
-    ScanVal e = sv_add(warp_exclusive_scan_small(v), blk);
+    const ScanVal blk = agg_combine(p.sub_pre[i >> 5], agg_combine(p.tile_pre[tile], p.grp_pre[tile >> 10]));
+    ScanVal e = agg_combine(warp_exclusive_scan_small(v), blk);
     const uint64_t tp = 1 + (uint64_t)e.w;  // slot 0 is the first root word
     bool live = i < p.n;
     if (live && tp + v.w > p.tape_cap) {
@@ -1277,6 +1259,7 @@ __global__ void __launch_bounds__(S2_THREADS) s2_grammar_kernel(const Stage2Para
 // ---------------------------------------------------------------------------------
 // K2f: root words.  Record r opens at rootpos[r]; its close sits right before the next
 // record's open (or is the last word of the tape).  stage2...go:170,207-218,428-441
+// (s2s_link_kernel writes the same words for the streaming path, bounded by tape_len instead of tape_cap)
 // ---------------------------------------------------------------------------------
 __global__ void s2_roots_kernel(const Stage2Params p, uint64_t n_records, uint64_t tape_len) {
     const uint64_t r = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;

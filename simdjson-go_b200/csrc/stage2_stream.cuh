@@ -2,7 +2,8 @@
 //
 //   K2p s2s_count      one warp per 6 KiB slab: per-slab aggregate (tape words, string bytes, brackets, depth, records,
 //                      structurals, numbers, bytes behind the last quote)
-//   K2q s2s_scan_*     exclusive scan of the aggregates (groups of 1024 + their totals), grand totals -> Stage2Result
+//   K2q scan_*_kernel<SlabAgg> (stage2.cuh)   exclusive scan of the aggregates (groups of 1024 + their totals),
+//                      grand totals -> Stage2Result
 //   K2r s2s_emit       the same analysis again, now with every offset known: tape words, Strings.B bytes (compacted in
 //                      shared memory and streamed out with coalesced / 16-byte stores), bracket records for the scope
 //                      matching, number list, per-segment grammar masks
@@ -111,89 +112,6 @@ __global__ void __launch_bounds__(S2S_THREADS, S2S_EMIT_MIN_BLOCKS) s2s_emit_ker
     sm.cmptab = tabs.cmptab;
     DevWarp wp;
     s2s_warp_loop<DevWarp, true>(wp, p, blockIdx.x * S2S_WARPS + warp, gridDim.x * S2S_WARPS, sm);
-}
-
-// ---------------------------------------------------------------------------------
-// K2q: exclusive scan of SlabAgg with agg_combine (not commutative in `trail`)
-// ---------------------------------------------------------------------------------
-__device__ __forceinline__ SlabAgg agg_shfl_up(const SlabAgg& a, int d) {
-    SlabAgg r;
-    r.w = __shfl_up_sync(FULL, a.w, d);
-    r.str = __shfl_up_sync(FULL, a.str, d);
-    r.brk = __shfl_up_sync(FULL, a.brk, d);
-    r.rec = __shfl_up_sync(FULL, a.rec, d);
-    r.depth = __shfl_up_sync(FULL, a.depth, d);
-    r.ns = __shfl_up_sync(FULL, a.ns, d);
-    r.num = __shfl_up_sync(FULL, a.num, d);
-    r.trail = __shfl_up_sync(FULL, a.trail, d);
-    return r;
-}
-// blockDim.x = 1024; returns the exclusive prefix of the calling thread, `total` = the block's sum
-__device__ __forceinline__ SlabAgg block_exclusive_scan_agg(const SlabAgg& v, SlabAgg& total) {
-    __shared__ SlabAgg warp_inc[33];
-    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-    SlabAgg inc = v;
-#pragma unroll
-    for (int d = 1; d < 32; d <<= 1) {
-        const SlabAgg t = agg_shfl_up(inc, d);
-        if (lane >= d) inc = agg_combine(t, inc);
-    }
-    if (lane == 31) warp_inc[warp + 1] = inc;
-    __syncthreads();
-    if (warp == 0) {
-        SlabAgg wv = warp_inc[lane + 1];  // 32 warps
-#pragma unroll
-        for (int d = 1; d < 32; d <<= 1) {
-            const SlabAgg t = agg_shfl_up(wv, d);
-            if (lane >= d) wv = agg_combine(t, wv);
-        }
-        __syncwarp();
-        warp_inc[lane + 1] = wv;  // inclusive over warps <= lane
-        if (lane == 0) warp_inc[0] = agg_zero();
-    }
-    __syncthreads();
-    total = warp_inc[32];
-    SlabAgg ex = agg_shfl_up(inc, 1);
-    if (lane == 0) ex = agg_zero();
-    const SlabAgg r = agg_combine(warp_inc[warp], ex);
-    __syncthreads();  // the shared array is reused by the next call
-    return r;
-}
-
-__global__ void __launch_bounds__(1024) s2s_scan_groups_kernel(const SlabAgg* in, uint32_t n, SlabAgg* pre, SlabAgg* group_total) {
-    const uint32_t i = blockIdx.x * 1024 + threadIdx.x;
-    const SlabAgg v = i < n ? in[i] : agg_zero();
-    SlabAgg total;
-    const SlabAgg e = block_exclusive_scan_agg(v, total);
-    if (i < n) pre[i] = e;
-    if (threadIdx.x == 0) group_total[blockIdx.x] = total;
-}
-
-__global__ void __launch_bounds__(1024) s2s_scan_top_kernel(const SlabAgg* in, uint32_t n, SlabAgg* pre, Stage2Result* res,
-                                                            uint64_t* totals_out, uint64_t msg_bytes) {
-    SlabAgg carry = agg_zero();
-    for (uint32_t base = 0; base < n; base += 1024) {
-        const uint32_t i = base + threadIdx.x;
-        const SlabAgg v = i < n ? in[i] : agg_zero();
-        SlabAgg total;
-        const SlabAgg e = block_exclusive_scan_agg(v, total);
-        if (i < n) pre[i] = agg_combine(carry, e);
-        carry = agg_combine(carry, total);
-    }
-    if (threadIdx.x == 0) {
-        res->tape_len = (uint64_t)carry.w + 2;  // + root open + root close
-        res->strings_len = carry.str;
-        res->n_brackets = carry.brk;
-        res->n_records = carry.rec;
-        res->final_depth = carry.depth;
-        res->n_numbers = carry.num;
-        if (totals_out) {  // sj_shard_totals in device memory, for an exchange that stays on the stream
-            totals_out[0] = msg_bytes;
-            totals_out[1] = (uint64_t)carry.w + 2;
-            totals_out[2] = carry.str;
-            totals_out[3] = (uint64_t)carry.rec + 1;
-        }
-    }
 }
 
 // ---------------------------------------------------------------------------------

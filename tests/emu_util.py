@@ -14,7 +14,7 @@ _lib = None
 
 
 def build(force=False):
-    deps = [_SRC] + [os.path.join(_CSRC, f) for f in ("s2s_core.h", "s2s_slab.h")]
+    deps = [_SRC] + [os.path.join(_CSRC, f) for f in ("bits.h", "s2s_core.h", "s2s_slab.h")]
     if force or not os.path.exists(_LIB) or any(os.path.getmtime(d) > os.path.getmtime(_LIB) for d in deps):
         subprocess.check_call(["g++", "-O2", "-g", "-std=c++17", "-shared", "-fPIC", "-Wall", "-Wno-unknown-pragmas"] + _FLAGS + ["-o", _LIB, _SRC])
 
