@@ -1,10 +1,28 @@
-// context.cuh -- per-context CUDA stream, events and grow-only device scratch.
+// context.cuh -- per-context CUDA stream, events, result block and grow-only device scratch.
 #pragma once
+#include <cstddef>
 #include <cstdint>
 #include <cstdlib>
 #include <cuda_runtime.h>
 
 #include "common.cuh"
+#include "stage1.cuh"
+#include "stage2_common.cuh"
+
+// The context's result block: one device allocation (sj_ctx::result) and its pinned mirror (sj_ctx::host_result).  The
+// kernels write s1 and s2; read_back copies a byte range of it to the mirror.
+struct ResultBlock {
+    sj::Stage1Result s1;
+    uint8_t gap1[64 - sizeof(sj::Stage1Result)];
+    sj::Stage2Result s2;
+    uint8_t gap2[128 - sizeof(sj::Stage2Result)];
+    uint64_t counters[2];  // mirror only: where the tape consumers (sj_consume.inl) land their two device counters
+};
+static_assert(offsetof(ResultBlock, s1) == 0, "result block layout");
+static_assert(offsetof(ResultBlock, s2) == 64, "result block layout");
+static_assert(offsetof(ResultBlock, counters) == 192, "result block layout");
+
+struct S2Pending;  // sj_parse.inl
 
 struct DevBuf {
     void* p = nullptr;
@@ -49,12 +67,12 @@ struct sj_ctx {
     DevBuf idx;      // structural positions (uint32)
     DevBuf desc;     // K1 look-back descriptors (one 128-byte slot per tile and chain) + per-tile slab in-string bits
     const uint32_t* last_slabpar = nullptr;  // the in-string bits of the last stage-1 launch (inside desc), or null
-    DevBuf result;   // Stage1Result + Stage2Result
-    void* host_result = nullptr;  // pinned mirror
+    DevBuf result;                        // ResultBlock
+    ResultBlock* host_result = nullptr;   // its pinned mirror
     // stage 2
-    void* pending = nullptr;  // S2Pending (sj_parse.inl): state between the counting and the emitting half of stage 2
+    S2Pending* pending = nullptr;  // state between the counting and the emitting half of stage 2
     int s2_impl = 0;  // stage 2: 0 = streaming kernels (stage2_stream.cuh) when copy_strings is on, 1 = per-structural kernels (stage2.cuh) always
-    DevBuf s2a, s2b, s2c, s2d, s2e, s2f, s2g;  // s2a/s2b: stage-2 scratch (before / after the totals are known), s2c: backslash block map
+    DevBuf s2a, s2b, s2c;  // s2a/s2b: stage-2 scratch (before / after the totals are known), s2c: backslash block map
     DevBuf tape, strings;  // device outputs for the host-buffer API
     // tape consumers (consume.cuh): needles + counters, root list of a foreign tape
     DevBuf tc_small, tc_roots;

@@ -2,8 +2,9 @@
 //
 // Host logic here mirrors the reference's parse driver (parse_json_amd64.go:28-127) and
 // stage-1 driver epilogue (stage1_find_marks_amd64.go:115-148); all byte work runs in the
-// sm_90a kernels of stage1.cuh / stage2.cuh.  There is NO CPU fallback: without a CUDA
-// device every entry point returns SJ_ERR_NO_DEVICE.
+// sm_90a kernels of stage1.cuh and of the two stage-2 implementations (stage2_stream.cuh,
+// stage2.cuh; what both run is in stage2_common.cuh).  There is NO CPU fallback: without a
+// CUDA device every entry point returns SJ_ERR_NO_DEVICE.
 #include <chrono>
 #include <cstdio>
 #include <cstdlib>
@@ -17,8 +18,8 @@
 #include "../../include/simdjson_b200.h"
 #include "context.cuh"
 #include "stage1.cuh"
-#include "stage2.cuh"
 #include "stage2_stream.cuh"
+#include "stage2.cuh"
 #include "consume.cuh"
 #include "gen.cuh"
 #include "exchange.cuh"
@@ -138,6 +139,7 @@ extern "C" const char* sj_error_string(int rc) {
 
 extern "C" void sj_ctx_destroy(sj_ctx* c);
 static void exchange_release(sj_ctx* c);  // sj_exchange.inl
+static S2Pending* s2_pending_alloc();     // sj_parse.inl
 
 extern "C" int sj_ctx_create(int device, sj_ctx** out) {
     if (!out) return SJ_ERR_ARGUMENT;
@@ -162,9 +164,11 @@ extern "C" int sj_ctx_create(int device, sj_ctx** out) {
         c->stream = c->own_stream;
         SJ_CUDA_CHECK(cudaEventCreate(&c->ev[0]));
         SJ_CUDA_CHECK(cudaEventCreate(&c->ev[1]));
-        SJ_CUDA_CHECK(cudaHostAlloc(&c->host_result, 256, cudaHostAllocDefault));
-        int r = c->result.reserve(256);
+        SJ_CUDA_CHECK(cudaHostAlloc(&c->host_result, sizeof(ResultBlock), cudaHostAllocDefault));
+        int r = c->result.reserve(sizeof(ResultBlock));
         if (r) return r;
+        c->pending = s2_pending_alloc();
+        if (!c->pending) return SJ_ERR_ARGUMENT;
         SJ_CUDA_CHECK(cudaFuncSetAttribute(stage1_flatten_kernel<false, false>, cudaFuncAttributeMaxDynamicSharedMemorySize,
                                            (int)S1_SMEM_BYTES));
         SJ_CUDA_CHECK(cudaFuncSetAttribute(stage1_flatten_kernel<false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize,
@@ -196,9 +200,8 @@ extern "C" void sj_ctx_destroy(sj_ctx* c) {
     cudaSetDevice(c->device);
     if (c->stream) cudaStreamSynchronize(c->stream);
     exchange_release(c);
-    DevBuf* bufs[] = {&c->msg,  &c->idx, &c->desc, &c->result, &c->s2a,     &c->s2b,     &c->s2c,      &c->s2d,
-                      &c->s2e,  &c->s2f, &c->s2g,  &c->tape,   &c->strings, &c->test_in, &c->test_out, &c->test_aux,
-                      &c->tc_small, &c->tc_roots};
+    DevBuf* bufs[] = {&c->msg,     &c->idx,     &c->desc,    &c->result,   &c->s2a,      &c->s2b,      &c->s2c,
+                      &c->tape,    &c->strings, &c->test_in, &c->test_out, &c->test_aux, &c->tc_small, &c->tc_roots};
     for (DevBuf* b : bufs) b->release();
     if (c->host_result) cudaFreeHost(c->host_result);
     free(c->pending);
@@ -327,7 +330,8 @@ static int launch_stage1(sj_ctx* c, const uint8_t* d_msg, size_t len, bool ndjso
     int rc = c->desc.reserve(desc_bytes);
     if (rc) return rc;
     SJ_CUDA_CHECK(cudaMemsetAsync(c->desc.p, 0, desc_bytes, c->stream));
-    SJ_CUDA_CHECK(cudaMemsetAsync(c->result.p, 0, sizeof(Stage1Result), c->stream));
+    ResultBlock* const block = c->result.as<ResultBlock>();
+    SJ_CUDA_CHECK(cudaMemsetAsync(&block->s1, 0, sizeof(Stage1Result), c->stream));
     Stage1Params p;
     p.msg = d_msg;
     p.len = len;
@@ -336,12 +340,11 @@ static int launch_stage1(sj_ctx* c, const uint8_t* d_msg, size_t len, bool ndjso
     p.lastp1 = reinterpret_cast<uint32_t*>(c->desc.as<uint8_t>() + off_last);
     p.dpar = c->desc.as<uint8_t>() + off_par;
     p.dcnt = c->desc.as<uint8_t>() + off_cnt;
-    p.result = c->result.as<Stage1Result>();
+    p.result = &block->s1;
     p.ntiles = ntiles;
     p.bsmap = d_bsmap;
     p.slabpar = want_slabpar ? reinterpret_cast<uint32_t*>(c->desc.as<uint8_t>() + off_slab) : nullptr;
     c->last_slabpar = p.slabpar;
-    p.prof = reinterpret_cast<unsigned long long*>(c->result.as<uint8_t>() + 128);
     int grid = ntiles;
     if (grid > c->s1_max_ctas) grid = c->s1_max_ctas;
     // cooperative launch: the static tile deal needs every CTA of the grid resident at once
@@ -359,10 +362,11 @@ static int launch_stage1(sj_ctx* c, const uint8_t* d_msg, size_t len, bool ndjso
     return SJ_OK;
 }
 
-static int fetch_stage1_result(sj_ctx* c, Stage1Result* r) {
-    SJ_CUDA_CHECK(cudaMemcpyAsync(c->host_result, c->result.p, sizeof(Stage1Result), cudaMemcpyDeviceToHost, c->stream));
+// bytes [off, off + n) of the result block to the host, and the synchronisation that makes them valid there
+static int read_back(sj_ctx* c, size_t off, size_t n) {
+    SJ_CUDA_CHECK(cudaMemcpyAsync(reinterpret_cast<uint8_t*>(c->host_result) + off, c->result.as<uint8_t>() + off, n,
+                                  cudaMemcpyDeviceToHost, c->stream));
     SJ_CUDA_CHECK(cudaStreamSynchronize(c->stream));
-    memcpy(r, c->host_result, sizeof(Stage1Result));
     return SJ_OK;
 }
 
@@ -377,9 +381,9 @@ extern "C" int sj_stage1_device(sj_ctx* c, const uint8_t* d_msg, size_t len, int
     if (!c) return SJ_ERR_ARGUMENT;
     int rc = launch_stage1(c, d_msg, len, ndjson != 0, deltas != 0, d_out, cap);
     if (rc) return rc;
-    Stage1Result r;
-    rc = fetch_stage1_result(c, &r);
+    rc = read_back(c, offsetof(ResultBlock, s1), sizeof(Stage1Result));
     if (rc) return rc;
+    const Stage1Result r = c->host_result->s1;
     if (info) {
         info->n_idx = r.n_idx;
         info->error = r.error;
@@ -425,8 +429,9 @@ extern "C" int sj_find_structural_indices(sj_ctx* c, const uint8_t* msg, size_t 
         if (rc) return rc;
         rc = launch_stage1(c, c->msg.as<uint8_t>(), len, ndjson != 0, true, c->idx.as<uint32_t>(), dcap);
         if (rc) return rc;
-        rc = fetch_stage1_result(c, &r);
+        rc = read_back(c, offsetof(ResultBlock, s1), sizeof(Stage1Result));
         if (rc) return rc;
+        r = c->host_result->s1;
         if (!r.overflow) break;
         dcap = (size_t)r.n_idx + 64;
     }
@@ -521,19 +526,3 @@ extern "C" int sj_test_flatten_bits(sj_ctx* c, const uint64_t* masks, size_t nma
 #include "sj_consume.inl"
 #include "sj_stream.inl"
 #include "sj_gen.inl"
-
-#ifdef SJ_PROFILE_PHASES
-// development aid (not part of the C ABI): read / clear the per-phase cycle counters
-extern "C" int sj_debug_read_prof(sj_ctx* c, unsigned long long* out, int clear) {
-    unsigned long long* d = reinterpret_cast<unsigned long long*>(c->result.as<uint8_t>() + 128);
-    SJ_CUDA_CHECK(cudaStreamSynchronize(c->stream));
-    SJ_CUDA_CHECK(cudaMemcpy(out, d, 128, cudaMemcpyDeviceToHost));
-    if (clear) SJ_CUDA_CHECK(cudaMemset(d, 0, 128));
-    return SJ_OK;
-}
-extern "C" int sj_debug_read_timeline(sj_ctx* c, unsigned long long* out) {
-    SJ_CUDA_CHECK(cudaStreamSynchronize(c->stream));
-    SJ_CUDA_CHECK(cudaMemcpyFromSymbol(out, sj::g_timeline, sizeof(unsigned long long) * 8 * 256 * 4));
-    return SJ_OK;
-}
-#endif

@@ -107,9 +107,8 @@ __device__ __forceinline__ uint32_t gather4(uint32_t flags, uint32_t acc) {
 }
 
 // rotate a 64-bit mask left by 16*r bits (r = 0..3): undoes the bank-conflict-free
-// chunk rotation used when a lane reads its 64 bytes from shared memory
-// The same rotation as two PRMTs: the four 16-bit pieces of (lo, hi) are re-ordered by per-lane
-// selectors (rot_selectors) computed once per thread.
+// chunk rotation used when a lane reads its 64 bytes from shared memory.  Two PRMTs: the four
+// 16-bit pieces of (lo, hi) are re-ordered by per-lane selectors (rot_selectors) computed once per thread.
 struct RotSel {
     uint32_t lo, hi;
 };
@@ -123,18 +122,6 @@ __device__ __forceinline__ RotSel rot_selectors(uint32_t r) {
 }
 __device__ __forceinline__ uint64_t rotl16x(uint32_t lo, uint32_t hi, const RotSel& s) {
     return mk64(__byte_perm(lo, hi, s.lo), __byte_perm(lo, hi, s.hi));
-}
-__device__ __forceinline__ uint64_t rotl16x(uint64_t m, uint32_t r) {
-    uint32_t lo = (uint32_t)m, hi = (uint32_t)(m >> 32);
-    if (r & 2) {
-        uint32_t t = lo;
-        lo = hi;
-        hi = t;
-    }
-    uint32_t s = (r & 1) * 16;
-    uint32_t nlo = __funnelshift_l(hi, lo, s);
-    uint32_t nhi = __funnelshift_l(lo, hi, s);
-    return mk64(nlo, nhi);
 }
 
 struct BlockMasks {
@@ -566,23 +553,14 @@ __device__ __forceinline__ uint32_t* par_slot(uint8_t* dpar, int tile) {
 __device__ __forceinline__ uint8_t* cnt_slot(uint8_t* dcnt, int tile) { return dcnt + (size_t)tile * S1_DESC_STRIDE; }
 
 // quote parity of everything in front of `tile` (tile > 0)
-__device__ __forceinline__ uint32_t lookback_parity(uint8_t* dpar, int tile, unsigned long long* prof = nullptr) {
+__device__ __forceinline__ uint32_t lookback_parity(uint8_t* dpar, int tile) {
     const int lane = threadIdx.x & 31;
     uint32_t par = 0;
-#ifdef SJ_PROFILE_PHASES
-    unsigned long long nspin = 0, nround = 0;
-#endif
     for (int base = tile - 1;; base -= 32 * S1_LB_PER_LANE) {
         uint32_t d[S1_LB_PER_LANE];
         bool again = false;
         uint32_t ok;
-#ifdef SJ_PROFILE_PHASES
-        nround++;
-#endif
         do {
-#ifdef SJ_PROFILE_PHASES
-            nspin++;
-#endif
             if (again) __nanosleep(S1_SPIN_SLEEP_NS);
             again = true;
             ok = 1;
@@ -602,9 +580,6 @@ __device__ __forceinline__ uint32_t lookback_parity(uint8_t* dpar, int tile, uns
             } else {  // the nearest inclusive descriptor: it and everything nearer
                 const uint32_t f = __ffs(I) - 1;
                 par ^= __popc(P & (0xffffffffu >> (31 - f))) & 1;
-#ifdef SJ_PROFILE_PHASES
-                if (prof && lane == 0) atomicAdd(prof + 9, nspin), atomicAdd(prof + 10, nround);
-#endif
                 return par;
             }
         }
@@ -612,24 +587,15 @@ __device__ __forceinline__ uint32_t lookback_parity(uint8_t* dpar, int tile, uns
 }
 
 // number of structurals in all tiles in front of `tile` (tile > 0)
-__device__ __forceinline__ uint64_t lookback_count(uint8_t* dcnt, int tile, unsigned long long* prof = nullptr) {
+__device__ __forceinline__ uint64_t lookback_count(uint8_t* dcnt, int tile) {
     const int lane = threadIdx.x & 31;
     uint64_t total = 0;
-#ifdef SJ_PROFILE_PHASES
-    unsigned long long nspin = 0, nround = 0;
-#endif
     for (int base = tile - 1;; base -= 32 * S1_LB_PER_LANE) {
         uint32_t agg[S1_LB_PER_LANE];
         uint64_t inc[S1_LB_PER_LANE];
         bool again = false;
         uint32_t ok;
-#ifdef SJ_PROFILE_PHASES
-        nround++;
-#endif
         do {
-#ifdef SJ_PROFILE_PHASES
-            nspin++;
-#endif
             if (again) __nanosleep(S1_SPIN_SLEEP_NS);
             again = true;
             ok = DA_VALID;
@@ -657,9 +623,6 @@ __device__ __forceinline__ uint64_t lookback_count(uint8_t* dcnt, int tile, unsi
             total += v;
             if (I) {
                 const uint32_t lo = __shfl_sync(FULL, (uint32_t)inc[j], f), hi = __shfl_sync(FULL, (uint32_t)(inc[j] >> 32), f);
-#ifdef SJ_PROFILE_PHASES
-                if (prof && lane == 0) atomicAdd(prof + 12, nspin), atomicAdd(prof + 13, nround);
-#endif
                 return total + ((((uint64_t)hi << 32) | lo) & ~DI_VALID);
             }
         }
@@ -684,48 +647,6 @@ __device__ __forceinline__ uint32_t backslash_run_before(const uint8_t* __restri
     }
 }
 
-
-#ifdef SJ_PROFILE_PHASES
-// development aid: per-phase cycle totals (lane 0 of every warp), summed into prof[0..7]
-#define SJ_PROF_DECL unsigned long long prof_t0 = clock64(), prof_acc[8] = {0, 0, 0, 0, 0, 0, 0, 0};
-#define SJ_PROF_MARK(k)                                  \
-    {                                                    \
-        unsigned long long t_ = clock64();               \
-        prof_acc[k] += t_ - prof_t0;                     \
-        prof_t0 = t_;                                    \
-    }
-#define SJ_PROF_FLUSH                                                                   \
-    if (lane == 0)                                                                      \
-        for (int k_ = 0; k_ < 8; k_++) atomicAdd(p.prof + k_, prof_acc[k_]);
-#else
-#define SJ_PROF_DECL
-#define SJ_PROF_MARK(k)
-#define SJ_PROF_FLUSH
-#endif
-
-#ifdef SJ_PROFILE_PHASES
-// timeline of the scan warp of 8 CTAs (globaltimer ns): [cta][iteration][event]
-// events: 0 = chain 2 done, 1 = barrier (1) passed, 2 = chain 1 done, 3 = barrier (3) passed
-__device__ unsigned long long g_timeline[8][256][4];
-__device__ __forceinline__ unsigned long long globaltimer_ns() {
-    unsigned long long t;
-    asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t));
-    return t;
-}
-__device__ __forceinline__ int timeline_slot() {
-    const int c = blockIdx.x, G = gridDim.x;
-    if (c < 3) return c;
-    if (c == G / 2 - 1) return 3;
-    if (c == G / 2) return 4;
-    if (c >= G - 3) return 5 + (c - (G - 3));
-    return -1;
-}
-#define SJ_TL(ev)                                                                            \
-    if (lane == 0 && tl_slot >= 0 && tl_it < 256) g_timeline[tl_slot][tl_it][ev] = globaltimer_ns();
-#else
-#define SJ_TL(ev)
-#endif
-
 struct Stage1Params {
     const uint8_t* msg;  // 16-byte aligned, readable up to round_up(len, 16)
     uint64_t len;
@@ -738,7 +659,6 @@ struct Stage1Params {
     uint32_t* slabpar;   // optional: [ntiles] bit w = "inside a string" in front of slab w of the tile (handed to the streaming stage 2)
     Stage1Result* result;
     int ntiles;
-    unsigned long long* prof;  // [8] cycle totals when built with -DSJ_PROFILE_PHASES
 };
 
 __device__ __forceinline__ void load_block_words(const uint8_t* buf, uint32_t lane, uint32_t (&w)[16]) {
@@ -820,24 +740,11 @@ __global__ void __launch_bounds__(S1_THREADS, S1_CTAS_PER_SM) stage1_flatten_ker
         uint32_t prev_tile_count = 0, prev_par_out = 0;
         uint32_t prev_wbase = 0, prev_wlast = 0;  // lane w: structurals / last structural (+1) in the slabs below slab w
         uint32_t itpar = 0;                        // parity of the iteration = phase of the hand-shake barriers
-#ifdef SJ_PROFILE_PHASES
-        const int tl_slot = timeline_slot();
-        int tl_it = -1;
-#endif
         while (tile < p.ntiles || have_prev) {
             const bool cur = tile < p.ntiles;  // CTA-uniform
             uint64_t tb = 0;
-#ifdef SJ_PROFILE_PHASES
-            tl_it++;
-#endif
             if (have_prev) {  // every tile in front of prev_tile published its count one iteration ago
-#ifdef SJ_PROFILE_PHASES
-                unsigned long long lb_t1 = clock64();
-                if (prev_tile > 0) tb = lookback_count(p.dcnt, prev_tile, p.prof);
-                if (lane == 0) atomicAdd(p.prof + 11, clock64() - lb_t1);
-#else
                 if (prev_tile > 0) tb = lookback_count(p.dcnt, prev_tile);
-#endif
                 if (lane == 0) {
                     st_relaxed_u64(reinterpret_cast<uint64_t*>(cnt_slot(p.dcnt, prev_tile) + 8), DI_VALID | (tb + prev_tile_count));
                     if (prev_tile == p.ntiles - 1) {
@@ -852,9 +759,7 @@ __global__ void __launch_bounds__(S1_THREADS, S1_CTAS_PER_SM) stage1_flatten_ker
             }
             __syncwarp();
             if (lane == 0) mbar_arrive(bar_S);
-            SJ_TL(0)
             mbar_wait(bar_P, itpar);  // every worker has classified its slab: buffer b^1 (tile i-1) is dead
-            SJ_TL(1)
             if (lane == 0) issue(tile + G, b ^ 1);
             const uint32_t parbits = __ballot_sync(FULL, lane < S1_WARPS && s_par[lane < S1_WARPS ? lane : 0] != 0);
             const uint32_t tile_par = __popc(parbits) & 1;
@@ -863,13 +768,7 @@ __global__ void __launch_bounds__(S1_THREADS, S1_CTAS_PER_SM) stage1_flatten_ker
                 if (lane == 0)
                     st_relaxed_u32(par_slot(p.dpar, tile), DP_VALID | (tile == 0 ? DP_INCL : 0) | (tile_par ? DP_PAR : 0));
                 if (tile > 0) {
-#ifdef SJ_PROFILE_PHASES
-                    unsigned long long lb_t0 = clock64();
-                    tin = lookback_parity(p.dpar, tile, p.prof);
-                    if (lane == 0) atomicAdd(p.prof + 8, clock64() - lb_t0), atomicAdd(p.prof + 14, 1ull);
-#else
                     tin = lookback_parity(p.dpar, tile);
-#endif
                     if (lane == 0) st_relaxed_u32(par_slot(p.dpar, tile), DP_VALID | DP_INCL | ((tile_par ^ tin) ? DP_PAR : 0));
                 }
             }
@@ -881,10 +780,8 @@ __global__ void __launch_bounds__(S1_THREADS, S1_CTAS_PER_SM) stage1_flatten_ker
             }
             __syncwarp();
             if (lane == 0) mbar_arrive(bar_Q);
-            SJ_TL(2)
             mbar_wait(bar_R, itpar);
             itpar ^= 1;
-            SJ_TL(3)
             // per-slab prefixes of the tile just finished (consumed by its flatten, next iteration)
             const uint32_t cnt = lane < S1_WARPS ? s_cnt[lane] : 0, l1 = lane < S1_WARPS ? s_last[lane] : 0;
             uint32_t incl = cnt;
@@ -914,7 +811,6 @@ __global__ void __launch_bounds__(S1_THREADS, S1_CTAS_PER_SM) stage1_flatten_ker
         return;
     }
 
-    SJ_PROF_DECL
     uint32_t phasebits = 0;
     uint32_t itpar = 0;  // parity of the iteration = phase of the hand-shake barriers
     const RotSel rsel = rot_selectors((lane >> 1) & 3);  // undoes the bank-conflict-free chunk order of load_block_words
@@ -937,7 +833,6 @@ __global__ void __launch_bounds__(S1_THREADS, S1_CTAS_PER_SM) stage1_flatten_ker
 
     while (tile < p.ntiles || have_prev) {
         const bool cur = tile < p.ntiles;  // CTA-uniform
-        SJ_PROF_MARK(7)
         const int slab = tile * S1_WARPS + (int)warp;
         const uint64_t slab_start = (uint64_t)slab * S1_SLAB_BYTES;
         const bool active = cur && slab_start < p.len;  // warps past the end of the message only keep the barriers
@@ -957,12 +852,10 @@ __global__ void __launch_bounds__(S1_THREADS, S1_CTAS_PER_SM) stage1_flatten_ker
             const uint32_t n = __ffs(~(peek_bs >> 1)) - 1;
             prevc_esc = n == 31 ? backslash_run_before(p.msg, slab_start - 1) & 1 : n & 1;
         }
-        SJ_PROF_MARK(7)
         if (cur) {
             mbar_wait(&bars[b], (phasebits >> b) & 1);
             phasebits ^= 1u << b;
         }
-        SJ_PROF_MARK(2)
 
         // the last tile: bytes past the end of the message read as spaces (find_structural_bits_amd64.s:167);
         // padded in shared memory so that the hot loop carries no tail handling at all
@@ -1029,7 +922,6 @@ __global__ void __launch_bounds__(S1_THREADS, S1_CTAS_PER_SM) stage1_flatten_ker
             s_par[warp] = slab_par;
             mbar_arrive(bar_P);
         }
-        SJ_PROF_MARK(3)
         const uint32_t peek_next = peek_load(tile + G);
         // ---------------- extraction of the previous tile's structurals ----------------
         // the positions are staged over the warp's own slab of this tile (dead: this warp alone read
@@ -1048,10 +940,8 @@ __global__ void __launch_bounds__(S1_THREADS, S1_CTAS_PER_SM) stage1_flatten_ker
                 }
             }
         }
-        SJ_PROF_MARK(4)
         mbar_wait(bar_S, itpar);  // output offsets of the previous tile (chain 2, run by the scan warp under phase A)
-        SJ_PROF_MARK(1)
-        __syncwarp();             // staged positions of all lanes are visible
+        __syncwarp();            // staged positions of all lanes are visible
 
         // ---------------- copy-out of the previous tile's staged structurals ----------------
         if (have_prev) {
@@ -1067,10 +957,8 @@ __global__ void __launch_bounds__(S1_THREADS, S1_CTAS_PER_SM) stage1_flatten_ker
                 flatten_slab_staged<DELTAS, S1_STEPS>(S_prev, pslab_pos, p.out + off, prev_last, stage, S1_SLAB_BYTES / 4);
             }
         }
-        SJ_PROF_MARK(5)
         mbar_wait(bar_Q, itpar);  // quote parity in front of the tile (chain 1, run by the scan warp meanwhile)
         const uint32_t par_in = s_parin[warp];
-        SJ_PROF_MARK(0)
 
         // pseudo-structural predecessor carry into the slab (finalize_structurals_amd64.s:24-27;
         // initial value 1: stage1_find_marks_amd64.go:54)
@@ -1123,7 +1011,6 @@ __global__ void __launch_bounds__(S1_THREADS, S1_CTAS_PER_SM) stage1_flatten_ker
             s_cnt[warp] = slab_count;
             s_last[warp] = own_last1;
         }
-        SJ_PROF_MARK(6)
         // R: slab counts of the tile are written (the same lane 0 wrote them)
         if (lane == 0) mbar_arrive(bar_R);
         itpar ^= 1;
@@ -1135,7 +1022,6 @@ __global__ void __launch_bounds__(S1_THREADS, S1_CTAS_PER_SM) stage1_flatten_ker
         tile += G;
         b ^= 1;
     }
-    SJ_PROF_FLUSH
 }
 
 // After K1: rebase the first delta of every tile on the last structural of the tiles in

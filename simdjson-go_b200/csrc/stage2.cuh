@@ -6,20 +6,19 @@
 //   K2a classify_measure  type of each structural, atom validation (stage2...go:124-158),
 //                         string validate-only pass (parse_string_amd64.s:72-258)
 //                         -> per-structural tape-word / bracket / string-byte / record counts
-//   K2b scans             exclusive prefix sums of those counts (tile sums -> 2-level scan)
+//   K2b scans             exclusive prefix sums of those counts (tile sums -> 2-level scan; stage2_common.cuh)
 //   K2c emit              tape slots, parse_number (parse_number.go:65), parse_string copy
 //                         (parse_string_amd64.s:260-479), bracket compaction
 //   K2d ansv              nearest-smaller-depth search over the brackets = the scope stack:
-//                         gives every close its open and every value its enclosing container
+//                         gives every close its open and every value its enclosing container (stage2_common.cuh)
 //   K2e grammar           the state machine's transition checks, evaluated locally from
 //                         (previous two structurals, enclosing container); cross-links { } [ ]
 //   K2f roots             root words and NDJSON root chaining (stage2...go:190-221, 428-441)
 #pragma once
-#include <type_traits>
-
 #include "common.cuh"
 #include "number.cuh"
 #include "s2s_core.h"
+#include "stage2_common.cuh"
 
 namespace sj {
 
@@ -28,7 +27,6 @@ namespace sj {
 constexpr uint32_t AUX_COPY = 0x80000000u;              // string goes to the string buffer
 constexpr uint32_t AUX_ESC = 0x40000000u;               // string contains escapes (source length != unescaped length)
 constexpr uint32_t AUX_LEN = 0x3fffffffu;
-constexpr int S2_THREADS = 256;
 constexpr int S2_ITEMS = 4;                       // consecutive structurals per thread in K2a / K2c / K2e
 constexpr int S2_TILE = S2_THREADS * S2_ITEMS;     // structurals per block = granularity of the K2b scan
 // Strings that need the byte-exact slow paths (escapes, or no escape-free proof from K1's backslash
@@ -72,55 +70,8 @@ __device__ __forceinline__ ScanVal agg_shfl_up(const ScanVal& a, int d) {
     r.depth = __shfl_up_sync(FULL, a.depth, d);
     return r;
 }
-__device__ __forceinline__ SlabAgg agg_shfl_up(const SlabAgg& a, int d) {
-    SlabAgg r;
-    r.w = __shfl_up_sync(FULL, a.w, d);
-    r.str = __shfl_up_sync(FULL, a.str, d);
-    r.brk = __shfl_up_sync(FULL, a.brk, d);
-    r.rec = __shfl_up_sync(FULL, a.rec, d);
-    r.depth = __shfl_up_sync(FULL, a.depth, d);
-    r.ns = __shfl_up_sync(FULL, a.ns, d);
-    r.num = __shfl_up_sync(FULL, a.num, d);
-    r.trail = __shfl_up_sync(FULL, a.trail, d);
-    return r;
-}
 
-// block-wide exclusive scan of ScanVal (K2b) or SlabAgg (K2q), blockDim.x = 1024; returns the exclusive prefix of the
-// calling thread and the block total.  agg_combine(a, b) puts a in front of b (SlabAgg's is not commutative in
-// `trail`).  Warp totals are scanned by the first warp so every thread reads just two entries of shared memory.
-template <class T>
-__device__ __forceinline__ T block_exclusive_scan(const T& v, T& total) {
-    __shared__ T warp_inc[33];  // [w] = sum of warps < w, [32] = block total
-    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-    T inc = v;
-#pragma unroll
-    for (int d = 1; d < 32; d <<= 1) {
-        const T t = agg_shfl_up(inc, d);
-        if (lane >= d) inc = agg_combine(t, inc);
-    }
-    if (lane == 31) warp_inc[warp + 1] = inc;  // provisional: the warp's own total
-    __syncthreads();
-    if (warp == 0) {
-        T wv = warp_inc[lane + 1];
-#pragma unroll
-        for (int d = 1; d < 32; d <<= 1) {
-            const T t = agg_shfl_up(wv, d);
-            if (lane >= d) wv = agg_combine(t, wv);
-        }
-        __syncwarp();
-        warp_inc[lane + 1] = wv;  // inclusive over warps <= lane
-        if (lane == 0) warp_inc[0] = T{};
-    }
-    __syncthreads();
-    total = warp_inc[32];
-    T ex = agg_shfl_up(inc, 1);
-    if (lane == 0) ex = T{};
-    const T r = agg_combine(warp_inc[warp], ex);
-    __syncthreads();  // the shared array is reused by the next call
-    return r;
-}
-
-// The same scan for the per-structural contributions of ONE block (K2a, K2c): every field but
+// The block scan of stage2_common.cuh for the per-structural contributions of ONE block (K2a, K2c): every field but
 // `str` is tiny (w <= 2, brk, rec <= 1, depth in {-1,0,1} per structural), so four of the five
 // fields travel as 16-bit lanes of one 64-bit word (depth biased by +BIAS per thread, BIAS = number
 // of structurals a thread contributes) and the scan moves 3 registers per step instead of 5.
@@ -215,18 +166,6 @@ __device__ __forceinline__ ScanVal warp_exclusive_scan_small(const ScanVal& v) {
     r.str = st - v.str;
     return r;
 }
-
-struct Stage2Result {
-    uint64_t tape_len;     // total tape words (including both root words of the last record)
-    uint64_t strings_len;  // bytes of the string buffer
-    uint64_t n_brackets;
-    uint64_t n_records;    // record boundaries (roots - 1)
-    int64_t final_depth;
-    uint32_t error;        // any stage-2 failure
-    uint32_t overflow;     // tape / string capacity exceeded
-    uint32_t n_numbers;    // structurals that start a number (K2a)
-    uint32_t num_fill;     // fill pointer of the number list (K2g)
-};
 
 struct Stage2Params {
     const uint8_t* msg;
@@ -365,7 +304,7 @@ __device__ __forceinline__ bool string_measure(const StrCursor& s, uint64_t max_
 }
 
 // _parse_string (parse_string_amd64.s:260-479) for a string that already validated.  The UTF-8 bytes of an escape are
-// stored one by one here and in the warp routines below: packing them with utf8_pack (bits.h) changes those stores.
+// stored one by one here and in warp_string_fast below: packing them with utf8_pack (bits.h) changes those stores.
 __device__ __forceinline__ void string_copy(const StrCursor& s, uint8_t* dst) {
     uint64_t p = 0, dl = 0;
     for (;;) {
@@ -397,7 +336,7 @@ __device__ __forceinline__ void string_copy(const StrCursor& s, uint8_t* dst) {
     }
 }
 
-// ---- the same two routines executed by a whole warp for ONE string (all 32 lanes call them with
+// ---- string_measure executed by a whole warp for ONE string (all 32 lanes call it with
 // identical arguments; control flow is warp-uniform).  The reference's assembly works on 32-byte
 // windows too (parse_string_amd64.s:84-100, 272-290): a window is loaded, the first '"' or '\\' in
 // it decides what happens next.  Here lane j holds byte j of the window and two ballots replace
@@ -430,46 +369,7 @@ __device__ __forceinline__ bool warp_string_measure(const StrCursor& s, uint64_t
     }
 }
 
-__device__ __forceinline__ void warp_string_copy(const StrCursor& s, uint8_t* dst) {
-    const uint32_t lane = threadIdx.x & 31;
-    uint64_t p = 0, dl = 0;
-    for (;;) {
-        const uint32_t c = s.at(p + lane);
-        const uint32_t qm = __ballot_sync(FULL, c == '"'), ev = qm | __ballot_sync(FULL, c == '\\');
-        const uint32_t j = ev ? __ffs(ev) - 1 : 32;
-        if (lane < j) dst[dl + lane] = (uint8_t)c;  // the plain bytes in front of the first event
-        if (ev == 0) {
-            p += 32;
-            dl += 32;
-            continue;
-        }
-        if ((qm >> j) & 1) return;
-        uint32_t adv, cp, n;
-        if (!escape_step(s, p + j, &adv, &cp, &n)) return;  // cannot happen after validation
-        if (lane == 0) {
-            uint8_t* o = dst + dl + j;
-            if (n == 1) {
-                o[0] = (uint8_t)cp;
-            } else if (n == 2) {
-                o[0] = (uint8_t)(0xC0 + (cp >> 6));
-                o[1] = (uint8_t)(0x80 | (cp & 63));
-            } else if (n == 3) {
-                o[0] = (uint8_t)(0xE0 + (cp >> 12));
-                o[1] = (uint8_t)(0x80 | ((cp >> 6) & 63));
-                o[2] = (uint8_t)(0x80 | (cp & 63));
-            } else {
-                o[0] = (uint8_t)(0xF0 + (cp >> 18));
-                o[1] = (uint8_t)(0x80 | ((cp >> 12) & 63));
-                o[2] = (uint8_t)(0x80 | ((cp >> 6) & 63));
-                o[3] = (uint8_t)(0x80 | (cp & 63));
-            }
-        }
-        dl += j + n;
-        p += j + adv;
-    }
-}
-
-// ---- all escapes of a 32-byte window at once.  The two routines above pay one window (load, two
+// ---- all escapes of a 32-byte window at once.  warp_string_measure pays one window (load, two
 // ballots, a redundant decode) per ESCAPE; text that is escaped character by character (twitterescaped:
 // "\u30c6\u30b9\u30c8...") makes that one window per six bytes.  Here every lane decodes "the escape
 // that would start at my byte" from its neighbours (shuffles), the lanes that really start one are
@@ -481,7 +381,8 @@ __device__ __forceinline__ void warp_string_copy(const StrCursor& s, uint8_t* ds
 //   * only starts at lanes <= 20 are decoded (a pair needs 12 bytes); the window is consumed up to
 //     the closing quote or up to the first undecoded start (>= lane 21), whichever comes first;
 //   * two high surrogates six bytes apart make "which one is the second half" a chain: such a
-//     window takes one exact step instead (warp_string_copy's step), as does nothing else.
+//     window takes one exact step instead (escape_step on the window's first event, as in
+//     warp_string_measure), as does nothing else.
 // Returns 0 = invalid, 1 = done (src_len / dst_len set), 2 = `bound` source bytes passed without a
 // closing quote (the caller lets the exact routine decide).  The exact routines above stay the
 // reference: the test hook runs all versions on every input. ----
@@ -843,49 +744,6 @@ __global__ void __launch_bounds__(S2_THREADS) s2_classify_measure_kernel(const S
 }
 
 // ---------------------------------------------------------------------------------
-// K2b (ScanVal per tile) / K2q (SlabAgg per slab): exclusive scan of `in[0..n)` in groups of 1024 (one block per group)
-// ---------------------------------------------------------------------------------
-template <class T>
-__global__ void __launch_bounds__(1024) scan_groups_kernel(const T* in, uint32_t n, T* pre, T* group_total) {
-    const uint32_t i = blockIdx.x * 1024 + threadIdx.x;
-    const T v = i < n ? in[i] : T{};
-    T total;
-    const T e = block_exclusive_scan(v, total);
-    if (i < n) pre[i] = e;
-    if (threadIdx.x == 0) group_total[blockIdx.x] = total;
-}
-
-// single block: exclusive scan of all group totals (looping), grand totals into `res` and, when given, into
-// `totals_out` (sj_shard_totals in device memory, for an exchange that stays on the stream)
-template <class T>
-__global__ void __launch_bounds__(1024) scan_top_kernel(const T* in, uint32_t n, T* pre, Stage2Result* res, uint64_t* totals_out,
-                                                        uint64_t msg_bytes) {
-    T carry{};
-    for (uint32_t base = 0; base < n; base += 1024) {
-        const uint32_t i = base + threadIdx.x;
-        const T v = i < n ? in[i] : T{};
-        T total;
-        const T e = block_exclusive_scan(v, total);
-        if (i < n) pre[i] = agg_combine(carry, e);
-        carry = agg_combine(carry, total);
-    }
-    if (threadIdx.x == 0) {
-        res->tape_len = (uint64_t)carry.w + 2;  // + root open + root close
-        res->strings_len = carry.str;
-        res->n_brackets = carry.brk;
-        res->n_records = carry.rec;
-        res->final_depth = carry.depth;
-        if constexpr (std::is_same<T, SlabAgg>::value) res->n_numbers = carry.num;  // (K2a adds up its own count)
-        if (totals_out) {
-            totals_out[0] = msg_bytes;
-            totals_out[1] = (uint64_t)carry.w + 2;
-            totals_out[2] = carry.str;
-            totals_out[3] = (uint64_t)carry.rec + 1;
-        }
-    }
-}
-
-// ---------------------------------------------------------------------------------
 // K2c
 // ---------------------------------------------------------------------------------
 // One structural per thread, warps independent of each other: with four structurals per thread the
@@ -1067,80 +925,6 @@ __global__ void __launch_bounds__(S2_THREADS) s2_numbers_kernel(const Stage2Para
     if (tag == 0) atomicOr(&p.result->error, 1u);
     p.tape[tp] = tag;
     p.tape[tp + 1] = val;
-}
-
-// ---------------------------------------------------------------------------------
-// K2d: min hierarchy + nearest-smaller-to-the-left
-// ---------------------------------------------------------------------------------
-constexpr int ANSV_MAX_LEVELS = 8;
-struct AnsvLevels {
-    const int32_t* lv[ANSV_MAX_LEVELS];
-    uint32_t n[ANSV_MAX_LEVELS];
-    int nlevels;
-};
-
-__global__ void s2_min32_kernel(const int32_t* in, uint32_t n_in, int32_t* out, uint32_t n_out) {
-    const uint32_t w = (blockIdx.x * blockDim.x + threadIdx.x) >> 5, lane = threadIdx.x & 31;
-    if (w >= n_out) return;
-    const uint32_t j = w * 32 + lane;
-    int32_t v = j < n_in ? in[j] : 0x7fffffff;
-#pragma unroll
-    for (int d = 16; d > 0; d >>= 1) v = min(v, __shfl_xor_sync(FULL, v, d));
-    if (lane == 0) out[w] = v;
-}
-
-__global__ void __launch_bounds__(S2_THREADS) s2_ansv_kernel(AnsvLevels L, int32_t* par) {
-    const uint32_t k = blockIdx.x * S2_THREADS + threadIdx.x;
-    if (k >= L.n[0]) return;
-    const int32_t* D = L.lv[0];
-    const int32_t t = D[k];
-    if (t <= 0) {
-        // nothing in front of a bracket at depth 0 can be shallower unless an earlier close went below the top level --
-        // which the grammar check rejects anyway (a close at the top level is in no legal transition), so the
-        // answer "none" is exact for every accepted document and harmless for the others.  (Every NDJSON record
-        // opens at depth 0: without this each of them walks the whole min hierarchy to find nothing.)
-        par[k] = -1;
-        return;
-    }
-    int64_t found = -1;
-    {
-        int64_t lo = k & ~31u;
-        for (int64_t m = (int64_t)k - 1; m >= lo; m--)
-            if (D[m] < t) {
-                found = m;
-                break;
-            }
-    }
-    if (found < 0) {
-        int lvl = 1;
-        int64_t idx = (int64_t)(k >> 5) - 1;
-        while (lvl < L.nlevels && idx >= 0) {
-            const int32_t* A = L.lv[lvl];
-            const int64_t lo = idx & ~31ll;
-            int64_t hit = -1;
-            for (int64_t j = idx; j >= lo; j--)
-                if (A[j] < t) {
-                    hit = j;
-                    break;
-                }
-            if (hit >= 0) {
-                int64_t cur = hit;
-                for (int l = lvl; l >= 1; l--) {  // descend: last child below the bound
-                    const int32_t* B = L.lv[l - 1];
-                    int64_t base = cur * 32, hi = base + 31;
-                    if (hi >= (int64_t)L.n[l - 1]) hi = (int64_t)L.n[l - 1] - 1;
-                    int64_t c = hi;
-                    while (c > base && !(B[c] < t)) c--;
-                    cur = c;
-                }
-                found = cur;
-                break;
-            }
-            idx = (lo >> 5) - 1;
-            lvl++;
-        }
-    }
-    par[k] = (int32_t)found;
 }
 
 // ---------------------------------------------------------------------------------

@@ -2,16 +2,15 @@
 //
 //   K2p s2s_count      one warp per 6 KiB slab: per-slab aggregate (tape words, string bytes, brackets, depth, records,
 //                      structurals, numbers, bytes behind the last quote)
-//   K2q scan_*_kernel<SlabAgg> (stage2.cuh)   exclusive scan of the aggregates (groups of 1024 + their totals),
-//                      grand totals -> Stage2Result
+//   K2q scan_*_kernel<SlabAgg> (stage2_common.cuh)   exclusive scan of the aggregates (groups of 1024 + their
+//                      totals), grand totals -> Stage2Result
 //   K2r s2s_emit       the same analysis again, now with every offset known: tape words, Strings.B bytes (compacted in
 //                      shared memory and streamed out with coalesced / 16-byte stores), bracket records for the scope
 //                      matching, number list, per-segment grammar masks
 //   K2h s2s_numbers    parse_number (parse_number.go:65) over the number list, one number per thread
-//   K2d s2_min32 + s2_ansv (stage2.cuh)    scope matching on the brackets
+//   K2d s2_min32 + s2_ansv (stage2_common.cuh)    scope matching on the brackets
 //   K2e s2s_link       per bracket: cross-links of { } [ ] (stage2...go:327-334) and the grammar verdict of the segment
-//                      in front of it against the container it lies in
-//   K2f s2_roots (stage2.cuh)
+//                      in front of it against the container it lies in; the same launch writes the root words (K2f)
 //
 // The unifiedMachine of the reference (stage2_build_tape_amd64.go:160-446) walks one structural at a time; the
 // per-structural kernels of stage2.cuh gave every structural a thread and spent ~460 warp-instructions per 32
@@ -22,7 +21,7 @@
 #include "number.cuh"
 #include "s2s_slab.h"
 #include "stage1.cuh"
-#include "stage2.cuh"
+#include "stage2_common.cuh"
 
 namespace sj {
 

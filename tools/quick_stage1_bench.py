@@ -46,15 +46,10 @@ for lib in libs:
     info = Info()
     rc = L.sj_stage1_device(h, d_msg.data_ptr(), n, 0, 0, d_out.data_ptr(), cap, C.byref(info))
     print(os.path.basename(lib), "rc", rc, "n_idx", info.n_idx, "err", info.error, "instr", info.ends_in_string)
-    has_prof = hasattr(L, "sj_debug_read_prof")
     for deltas in (0, 1):
         for it in range(3):
             L.sj_stage1_launch(h, d_msg.data_ptr(), n, 0, deltas, d_out.data_ptr(), cap)
         L.sj_ctx_sync(h)
-        if has_prof:
-            buf = (C.c_ulonglong * 16)()
-            L.sj_debug_read_prof.argtypes = [vp, C.c_void_p, C.c_int]
-            L.sj_debug_read_prof(h, buf, 1)
         reps = 10
         L.sj_event_record(h, 0)
         for it in range(reps):
@@ -65,21 +60,3 @@ for lib in libs:
         t = ms.value / reps / 1e3
         alg = n + 4 * info.n_idx
         print("  deltas=%d: %.3f ms  input %.1f GB/s  algorithmic %.1f GB/s" % (deltas, t * 1e3, n / t / 1e9, alg / t / 1e9))
-        if has_prof:
-            L.sj_debug_read_prof(h, buf, 1)
-            tot = float(sum(buf[:8]))
-            names = ["wait Q", "wait S", "tma wait", "phaseA", "extract", "copy-out", "phaseB", "top+peek"]
-            print("   " + "  ".join("%s %.1f%%" % (nm, 100 * v / tot) for nm, v in zip(names, buf)))
-            if hasattr(L, "sj_debug_read_timeline") and deltas == 0:
-                tl = (C.c_ulonglong * (8 * 256 * 4))()
-                L.sj_debug_read_timeline.argtypes = [vp, C.c_void_p]
-                L.sj_debug_read_timeline(h, tl)
-                import numpy as np
-                a = np.ctypeslib.as_array(tl).reshape(8, 256, 4).astype(np.int64)
-                t0 = a[:, 0, 1].min()
-                print("   timeline (us since first barrier(1)); per CTA slot: it: chain2done bar1 chain1done bar3")
-                for it in (0, 1, 2, 10, 11, 30, 31, 60, 61):
-                    print("   it %2d: " % it + " | ".join("%7.1f %7.1f %7.1f %7.1f" % tuple((a[c, it, :] - t0) / 1e3) for c in (0, 1, 3, 4, 6, 7)))
-            nt = max(1, buf[14])
-            print("   per tile: LB1 %.0f cyc, %.1f spins, %.2f rounds | LB2 %.0f cyc, %.1f spins, %.2f rounds | tiles %d" % (
-                buf[8] / nt, buf[9] / nt, buf[10] / nt, buf[11] / nt, buf[12] / nt, buf[13] / nt, buf[14]))
