@@ -188,6 +188,23 @@ int sj_parse_count_where(sj_ctx* ctx, const uint8_t* msg, size_t len, uint32_t f
                          size_t key_len, const uint8_t* value, size_t value_len, uint64_t* roots, uint64_t* matches);
 
 /*
+ * MarshalJSON on the device: Iter.MarshalJSON of a fresh pj.Iter() (parsed_json.go:394-556), byte for byte.  Every
+ * root's value as compact JSON, roots joined by one '\n' (no trailing newline); strings escaped like escapeBytes, floats
+ * like appendFloat (shortest round-trip digits; fixed notation for 1e-6 <= |x| < 1e21 and 0, else d.ddde+-N).
+ * sj_marshal_device: message, tape, strings and output in device memory; d_msg is only read for no-copy strings.  The
+ * tape is checked (tags, links of opens / closes / roots, string ranges, object keys, finite floats): a malformed one
+ * returns SJ_ERR_ARGUMENT and nothing outside the three inputs is read.  *out_len = bytes of the text, exact even on
+ * SJ_ERR_CAPACITY, when nothing is written.  A tape of length 0 gives 0 bytes.  Tapes longer than SJ_MAX_MARSHAL_TAPE
+ * words (the passes keep int32 depths and parents per word) return SJ_ERR_TOO_LARGE.
+ * sj_parse_marshal: HOST message in, parse and marshal on the device, only the text is copied to `out` (host memory);
+ * parse errors return the parse codes.
+ */
+#define SJ_MAX_MARSHAL_TAPE 0x7fffffffull
+int sj_marshal_device(sj_ctx* ctx, const uint8_t* d_msg, size_t msg_len, const uint64_t* d_tape, size_t tape_len,
+                      const uint8_t* d_strings, size_t strings_len, uint8_t* d_out, size_t cap, size_t* out_len);
+int sj_parse_marshal(sj_ctx* ctx, const uint8_t* msg, size_t len, uint32_t flags, uint8_t* out, size_t cap, size_t* out_len);
+
+/*
  * ParseNDStream (simdjson_amd64.go:116-215) inside the library: the caller pushes the bytes of an
  * NDJSON stream (any host memory, pageable included: they are staged once into pinned buffers),
  * the library cuts them at record boundaries into chunks of about `chunk_bytes` (:157-174; sized

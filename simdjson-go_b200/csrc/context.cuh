@@ -76,6 +76,8 @@ struct sj_ctx {
     DevBuf tape, strings;  // device outputs for the host-buffer API
     // tape consumers (consume.cuh): needles + counters, root list of a foreign tape
     DevBuf tc_small, tc_roots;
+    // device MarshalJSON (marshal.cuh): scratch of the passes, the text of sj_parse_marshal before its copy to the host
+    DevBuf mj, mj_out;
     // what the last successful stage 2 of this context left in device memory (valid until the next call)
     const uint32_t* last_rootpos = nullptr;  // stage 2's root list (slot of every record's root-open word, [0] implicit)
     uint64_t last_records = 0;               // record boundaries = roots - 1

@@ -21,6 +21,7 @@
 #include "stage2_stream.cuh"
 #include "stage2.cuh"
 #include "consume.cuh"
+#include "marshal.cuh"
 #include "gen.cuh"
 #include "exchange.cuh"
 
@@ -201,7 +202,8 @@ extern "C" void sj_ctx_destroy(sj_ctx* c) {
     if (c->stream) cudaStreamSynchronize(c->stream);
     exchange_release(c);
     DevBuf* bufs[] = {&c->msg,     &c->idx,     &c->desc,    &c->result,   &c->s2a,      &c->s2b,      &c->s2c,
-                      &c->tape,    &c->strings, &c->test_in, &c->test_out, &c->test_aux, &c->tc_small, &c->tc_roots};
+                      &c->tape,    &c->strings, &c->test_in, &c->test_out, &c->test_aux, &c->tc_small, &c->tc_roots,
+                      &c->mj,      &c->mj_out};
     for (DevBuf* b : bufs) b->release();
     if (c->host_result) cudaFreeHost(c->host_result);
     free(c->pending);
@@ -524,5 +526,6 @@ extern "C" int sj_test_flatten_bits(sj_ctx* c, const uint64_t* masks, size_t nma
 #include "sj_exchange.inl"
 #include "sj_parse.inl"
 #include "sj_consume.inl"
+#include "sj_marshal.inl"
 #include "sj_stream.inl"
 #include "sj_gen.inl"

@@ -156,3 +156,41 @@ func ParseAndCountWhere(msg []byte, ndjson bool, key, value string) (records, ma
 		return 0, 0, errors.New(C.GoString(C.sj_error_string(rc)))
 	}
 }
+
+// ParseAndMarshalJSON runs parseMessage and Iter.MarshalJSON (parsed_json.go:394-556) of the
+// whole tape in one call, with the tape left in device memory: the result is the compact JSON
+// text, one line per root, byte for byte what pj.Iter().MarshalJSON() returns.  Only the text
+// crosses PCIe.  The first attempt uses a buffer of len(msg)+64 bytes; if the text is longer,
+// the call is repeated once with the exact size it reported.
+func ParseAndMarshalJSON(msg []byte, ndjson bool) ([]byte, error) {
+	h := b200Get()
+	if h == nil {
+		return nil, errors.New("Host CPU does not meet target specs")
+	}
+	defer b200Put(h)
+	flags := C.uint32_t(C.SJ_FLAG_COPY_STRINGS)
+	if ndjson {
+		flags |= C.SJ_FLAG_NDJSON
+	}
+	var p *C.uint8_t
+	if len(msg) > 0 {
+		p = (*C.uint8_t)(unsafe.Pointer(&msg[0]))
+	}
+	out := make([]byte, len(msg)+64)
+	var n C.size_t
+	rc := C.sj_parse_marshal(h, p, C.size_t(len(msg)), flags, (*C.uint8_t)(unsafe.Pointer(&out[0])), C.size_t(len(out)), &n)
+	if rc == C.SJ_ERR_CAPACITY {
+		out = make([]byte, int(n)+1)
+		rc = C.sj_parse_marshal(h, p, C.size_t(len(msg)), flags, (*C.uint8_t)(unsafe.Pointer(&out[0])), C.size_t(len(out)), &n)
+	}
+	switch rc {
+	case C.SJ_OK:
+		return out[:int(n)], nil
+	case C.SJ_ERR_STAGE1:
+		return nil, errors.New("Failed to find all structural indices for stage 1")
+	case C.SJ_ERR_STAGE2:
+		return nil, errors.New("Bad parsing while executing stage 2")
+	default:
+		return nil, errors.New(C.GoString(C.sj_error_string(rc)))
+	}
+}

@@ -108,6 +108,47 @@ class Context:
             raise SjError(rc)
         return rc, roots.value, matches.value
 
+    def parse_marshal(self, msg, ndjson=False, copy_strings=True):
+        """parseMessage + Iter.MarshalJSON (parsed_json.go:394) with the tape left in HBM: (rc, JSON text bytes).  Only
+        the text is copied back; on a parse error the text is b""."""
+        m = _as_u8(msg)
+        flags = (FLAG_NDJSON if ndjson else 0) | (FLAG_COPY_STRINGS if copy_strings else 0)
+        n = C.c_size_t(0)
+        cap = m.size + 64  # compact text is rarely longer than its input; else once more at the exact size
+        for _ in range(2):
+            out = np.empty(max(cap, 1), dtype=np.uint8)
+            rc = self.L.sj_parse_marshal(self.h, _addr(m) if m.size else None, m.size, flags, _addr(out), cap, C.byref(n))
+            if rc != ERR_CAPACITY:
+                break
+            cap = n.value
+        if rc in (ERR_STAGE1, ERR_STAGE2):
+            return rc, b""
+        if rc != OK:
+            raise SjError(rc)
+        return rc, out[:n.value].tobytes()
+
+    def marshal_device(self, tape, strings=None, message=None, out=None):
+        """Iter.MarshalJSON of a tape already on this context's device: `tape` (int64 / uint64 torch tensor), `strings`
+        (Strings.B) and `message` (uint8 tensors, or None when empty).  Writes into `out` (uint8 tensor) or a new tensor.
+        Returns (rc, length of the text, the uint8 tensor view holding it); rc is SJ_ERR_CAPACITY when `out` is too small
+        (the length is still exact) and SJ_ERR_ARGUMENT for a malformed tape."""
+        import torch
+
+        def ptr_len(t):
+            return (t.data_ptr(), t.numel()) if t is not None and t.numel() else (None, 0)
+
+        sp, sl = ptr_len(strings)
+        mp, ml = ptr_len(message)
+        n = C.c_size_t(0)
+        if out is None:
+            rc = self.L.sj_marshal_device(self.h, mp, ml, tape.data_ptr(), tape.numel(), sp, sl, None, 0, C.byref(n))
+            if rc not in (OK, ERR_CAPACITY):
+                return rc, n.value, None
+            out = torch.empty(max(n.value, 1), dtype=torch.uint8, device=tape.device)
+        op, cap = out.data_ptr(), out.numel()
+        rc = self.L.sj_marshal_device(self.h, mp, ml, tape.data_ptr(), tape.numel(), sp, sl, op, cap, C.byref(n))
+        return rc, n.value, out[:n.value]
+
     # ---- unit-test hooks (same method names as oracle.pyoracle.Oracle) -----------
     def block_masks(self, blocks, carries):
         """blocks: (n,64) uint8; carries: (n,4) uint64 -> (n,12) uint64 (see simdjson_b200.h)."""

@@ -70,6 +70,34 @@ class Iter:
             return v
         return None
 
+    def MarshalJSON(self, ctx=None):
+        """Iter.MarshalJSON of a fresh Iter (parsed_json.go:394): the whole tape as compact JSON, one line per root.
+        The triple is uploaded and marshalled on the device (marshal.cuh) of `ctx` (default: the default context)."""
+        import numpy as np
+        import torch
+
+        from . import default_context
+        from ._lib import ERR_ARGUMENT, OK, SjError
+        ctx = ctx or default_context()
+        dev = torch.device("cuda", torch.cuda.current_device())
+
+        def up(a):
+            a = np.ascontiguousarray(a)
+            return torch.from_numpy(a.copy()).to(dev) if a.size else None
+
+        tape = up(np.asarray(self.tape, dtype=np.uint64).view(np.int64))
+        if tape is None:
+            return b""
+        strings = up(np.frombuffer(bytes(self.pj.Strings), dtype=np.uint8))
+        message = up(np.frombuffer(bytes(self.pj.Message), dtype=np.uint8))
+        torch.cuda.synchronize(dev)  # the library runs on its own stream
+        rc, n, out = ctx.marshal_device(tape, strings, message)
+        if rc == ERR_ARGUMENT:
+            raise ValueError("malformed tape")
+        if rc != OK:
+            raise SjError(rc)
+        return out.cpu().numpy().tobytes()
+
     def count_where(self, key, value):
         """ndjson_test.go:421 countWhere: records whose top-level `key` equals `value`."""
         return sum(1 for r in self.roots() if isinstance(r, dict) and r.get(key) == value)
