@@ -9,6 +9,7 @@ import subprocess
 import numpy as np
 import pytest
 
+from tests import fmt_values as fv
 from tests import marshal_oracle as mo
 from tests.util import SMALL_FILES, TAPE_FILES, golden, load_fixture, unhex
 
@@ -46,10 +47,6 @@ def _check_doubles(shim, bits):
         want = mo.format_float(struct.unpack("<d", struct.pack("<Q", b))[0])
         assert got == want, (hex(b), got, want)
     return len(bits)
-
-
-def _double_bits(xs):
-    return np.array([struct.unpack("<Q", struct.pack("<d", x))[0] for x in xs], dtype=np.uint64)
 
 
 def _oracle_tape(oracle, msg, ndjson, copy):
@@ -104,47 +101,26 @@ def test_doubles_in_the_fixture_tapes(shim, oracle):
 
 
 def test_powers_of_two_and_their_neighbours(shim):
-    xs = [math_ldexp(1.0, e) for e in range(-1074, 1024)]
-    b = _double_bits(xs)
-    allb = np.concatenate([b, b + np.uint64(1), b[1:] - np.uint64(1)])
-    allb = allb[(allb & np.uint64(0x7FF0000000000000)) != np.uint64(0x7FF0000000000000)]
-    assert _check_doubles(shim, np.concatenate([allb, allb | np.uint64(1 << 63)])) > 4000
-
-
-def math_ldexp(m, e):
-    import math
-    return math.ldexp(m, e)
+    assert _check_doubles(shim, fv.powers_of_two()) > 4000
 
 
 def test_notation_boundaries_and_integers(shim):
-    edges = _double_bits([1e-6, 1e21, 0.0, -0.0, 5e-324, 1.7976931348623157e308, 2.2250738585072014e-308, 0.1, 10.0,
-                          30886023086020860000.0, 9007199254740993.0, 1e20, 1e22, 1e-7, 123456789.0, -9876.54321])
-    near = np.concatenate([edges + np.uint64(d) for d in range(0, 4)] + [edges[edges > 4] - np.uint64(d) for d in range(1, 4)])
-    ints = _double_bits([float(k) for k in range(2 ** 53 - 1000, 2 ** 53 + 1000)] + [float(k) for k in range(-1000, 1000)])
-    pow10 = _double_bits([float("1e%d" % k) for k in range(-323, 309)])
-    near = near[(near & np.uint64(0x7FF0000000000000)) != np.uint64(0x7FF0000000000000)]
-    _check_doubles(shim, np.concatenate([near, ints, pow10, pow10 + np.uint64(1), pow10 - np.uint64(1)]))
+    _check_doubles(shim, np.concatenate([fv.notation_edges(), fv.integers_near_2_53(), fv.powers_of_ten()]))
 
 
 def test_a_million_random_bit_patterns(shim):
-    rng = np.random.default_rng(20260515)
-    b = rng.integers(0, 2 ** 64, size=1_100_000, dtype=np.uint64)
-    b = b[(b & np.uint64(0x7FF0000000000000)) != np.uint64(0x7FF0000000000000)]
-    assert len(b) >= 1_000_000
-    _check_doubles(shim, b)
-    # and doubles of ordinary magnitudes, where both notations and the shortening paths are dense
-    m = 10.0 ** rng.uniform(-30, 30, size=200_000) * np.sign(rng.uniform(-1, 1, size=200_000))
-    _check_doubles(shim, _double_bits([float("%.*g" % (int(p), x)) for p, x in zip(rng.integers(1, 18, size=m.size), m)]))
+    assert len(fv.random_bits()) >= 1_000_000
+    _check_doubles(shim, fv.random_bits())
+    _check_doubles(shim, fv.printf_g())
 
 
 def test_integers(shim):
-    vals = [0, 1, 9, 10, 99, 100, 2 ** 53, 2 ** 63 - 1, 2 ** 63, 2 ** 64 - 1] + [10 ** k + d for k in range(20) for d in (-1, 0, 1) if 0 <= 10 ** k + d < 2 ** 64]
-    v = np.array(vals, dtype=np.uint64)
+    v = np.array(fv.INTEGERS, dtype=np.uint64)
     for signed in (0, 1):
         out = np.zeros(32 * len(v), dtype=np.uint8)
         lens = np.zeros(len(v), dtype=np.uint32)
         shim.fmt_shim_ints(v.ctypes.data, len(v), signed, out.ctypes.data, lens.ctypes.data)
-        for x, got in zip(vals, _texts(out, lens)):
+        for x, got in zip(fv.INTEGERS, _texts(out, lens)):
             want = b"%d" % (x - (1 << 64) if signed and x >> 63 else x)
             assert got == want, (x, signed, got)
 
