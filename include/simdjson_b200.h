@@ -44,6 +44,7 @@ extern "C" {
 #define SJ_STREAM_BUSY 9  /* sj_stream_close_input: every slot is in use -- take a result first, then call again */
 #define SJ_ERR_EXCHANGE 10 /* sj_parse_nd_sharded_count: a peer's totals did not arrive within the exchange's time limit */
 #define SJ_ERR_PEER 11     /* sj_parse_nd_sharded_count: a peer's shard failed before its totals existed (the whole ParseND fails) */
+#define SJ_ERR_UNSUPPORTED 12 /* sj_deserialize_device: the stream has S2 or zstd blocks (read them on the CPU) */
 /* negative values: -(1000 + cudaError_t) */
 
 #define SJ_MAX_MESSAGE 0x7fffff00ull /* positions are uint32, string lengths keep one flag bit */
@@ -203,6 +204,33 @@ int sj_parse_count_where(sj_ctx* ctx, const uint8_t* msg, size_t len, uint32_t f
 int sj_marshal_device(sj_ctx* ctx, const uint8_t* d_msg, size_t msg_len, const uint64_t* d_tape, size_t tape_len,
                       const uint8_t* d_strings, size_t strings_len, uint8_t* d_out, size_t cap, size_t* out_len);
 int sj_parse_marshal(sj_ctx* ctx, const uint8_t* msg, size_t len, uint32_t flags, uint8_t* out, size_t cap, size_t* out_len);
+
+/*
+ * Serializer on the device: the v3 stream of Serializer.Serialize / Deserialize (parsed_serialize.go:200-695) with every
+ * block uncompressed (CompressNone), so the reference's NewSerializer().Deserialize reads what these write.  The one
+ * intended difference: strings are deduplicated exactly, keeping the first occurrence (the message block holds each
+ * distinct string once, in order of first appearance), where the reference's 16 K-bucket table keyed by a per-process
+ * seeded hash keeps some duplicates.  The stream does not depend on copy_strings.
+ * sj_serialize_device: message, tape, strings and output in device memory.  A tape the reference's Serialize panics on
+ * (an unknown tag, a string range outside its buffer, a string or number head as the last word) returns
+ * SJ_ERR_ARGUMENT; links are not checked.  *out_len is exact even on SJ_ERR_CAPACITY, when nothing is written.  An empty
+ * tape gives the 14-byte empty stream.  Tapes over SJ_MAX_MARSHAL_TAPE words return SJ_ERR_TOO_LARGE.
+ * sj_parse_serialize: HOST message in, parse and serialize on the device, only the stream is copied to `out` (host memory).
+ * sj_deserialize_device: stream in device memory to tape, Strings.B and message in device memory.  Accepted exactly when
+ * the reference's Deserialize on a zeroed tape returns no error and does not panic, every '{' / '[' names a later word
+ * that holds its matching close, and no close is named twice; the output then equals the reference's.  Versions 0-3 are
+ * read alike and bytes behind the values block are ignored.  S2 / zstd blocks return SJ_ERR_UNSUPPORTED, any other
+ * rejection SJ_ERR_ARGUMENT, over SJ_MAX_MARSHAL_TAPE tape words or tags SJ_ERR_TOO_LARGE.  The three sizes are exact on
+ * SJ_ERR_CAPACITY; nothing is written unless the call succeeds.
+ * sj_test_set_string_hash_bits: keep only `bits` bits of the dedup hash (0 = all), to force hash collisions in tests.
+ */
+int sj_serialize_device(sj_ctx* ctx, const uint8_t* d_msg, size_t msg_len, const uint64_t* d_tape, size_t tape_len,
+                        const uint8_t* d_strings, size_t strings_len, uint8_t* d_out, size_t cap, size_t* out_len);
+int sj_parse_serialize(sj_ctx* ctx, const uint8_t* msg, size_t len, uint32_t flags, uint8_t* out, size_t cap, size_t* out_len);
+int sj_deserialize_device(sj_ctx* ctx, const uint8_t* d_in, size_t in_len, uint64_t* d_tape, size_t tape_cap, size_t* tape_len,
+                          uint8_t* d_strings, size_t strings_cap, size_t* strings_len, uint8_t* d_msg, size_t msg_cap,
+                          size_t* msg_len);
+int sj_test_set_string_hash_bits(sj_ctx* ctx, int bits);
 
 /*
  * ParseNDStream (simdjson_amd64.go:116-215) inside the library: the caller pushes the bytes of an

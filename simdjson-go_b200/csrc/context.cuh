@@ -78,6 +78,9 @@ struct sj_ctx {
     DevBuf tc_small, tc_roots;
     // device MarshalJSON (marshal.cuh): scratch of the passes, the text of sj_parse_marshal before its copy to the host
     DevBuf mj, mj_out;
+    // device Serializer (serialize.cuh): scratch of the word passes, of the string dedup, the stream of sj_parse_serialize
+    DevBuf sz, sz_tab, sz_out;
+    uint32_t sz_hash_bits = 0;  // test hook: keep only this many bits of the dedup hash (0 = all)
     // what the last successful stage 2 of this context left in device memory (valid until the next call)
     const uint32_t* last_rootpos = nullptr;  // stage 2's root list (slot of every record's root-open word, [0] implicit)
     uint64_t last_records = 0;               // record boundaries = roots - 1

@@ -22,6 +22,7 @@
 #include "stage2.cuh"
 #include "consume.cuh"
 #include "marshal.cuh"
+#include "serialize.cuh"
 #include "gen.cuh"
 #include "exchange.cuh"
 
@@ -134,6 +135,7 @@ extern "C" const char* sj_error_string(int rc) {
     case SJ_STREAM_BUSY: return "every stream slot is in use";
     case SJ_ERR_EXCHANGE: return "sharded ParseND: a peer's totals did not arrive in time";
     case SJ_ERR_PEER: return "sharded ParseND: a peer's shard failed";
+    case SJ_ERR_UNSUPPORTED: return "serialized stream has S2 or zstd blocks: only uncompressed blocks are read on the device";
     default: return rc < 0 ? cudaGetErrorString((cudaError_t)(-rc - 1000)) : "unknown error";
     }
 }
@@ -203,7 +205,7 @@ extern "C" void sj_ctx_destroy(sj_ctx* c) {
     exchange_release(c);
     DevBuf* bufs[] = {&c->msg,     &c->idx,     &c->desc,    &c->result,   &c->s2a,      &c->s2b,      &c->s2c,
                       &c->tape,    &c->strings, &c->test_in, &c->test_out, &c->test_aux, &c->tc_small, &c->tc_roots,
-                      &c->mj,      &c->mj_out};
+                      &c->mj,      &c->mj_out,  &c->sz,      &c->sz_tab,   &c->sz_out};
     for (DevBuf* b : bufs) b->release();
     if (c->host_result) cudaFreeHost(c->host_result);
     free(c->pending);
@@ -527,5 +529,6 @@ extern "C" int sj_test_flatten_bits(sj_ctx* c, const uint64_t* masks, size_t nma
 #include "sj_parse.inl"
 #include "sj_consume.inl"
 #include "sj_marshal.inl"
+#include "sj_serialize.inl"
 #include "sj_stream.inl"
 #include "sj_gen.inl"

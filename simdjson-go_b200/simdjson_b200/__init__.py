@@ -10,7 +10,8 @@ import ctypes as C
 import numpy as np
 
 from . import _lib
-from ._lib import (ERR_CAPACITY, ERR_STAGE1, ERR_STAGE2, FLAG_COPY_STRINGS, FLAG_NDJSON, OK, SjError, Stage1Info)
+from ._lib import (ERR_CAPACITY, ERR_STAGE1, ERR_STAGE2, ERR_UNSUPPORTED, FLAG_COPY_STRINGS, FLAG_NDJSON, OK, SjError,
+                   Stage1Info)
 
 JSONVALUEMASK = 0xFF_FFFF_FFFF_FFFF  # parsed_json.go:26
 JSONTAGOFFSET = 56
@@ -149,6 +150,77 @@ class Context:
         rc = self.L.sj_marshal_device(self.h, mp, ml, tape.data_ptr(), tape.numel(), sp, sl, op, cap, C.byref(n))
         return rc, n.value, out[:n.value]
 
+    # ---- Serializer (parsed_serialize.go), uncompressed blocks ------------------
+    def parse_serialize(self, msg, ndjson=False, copy_strings=True):
+        """parseMessage + Serializer.Serialize (parsed_serialize.go:200) with the tape left in HBM: (rc, stream bytes).
+        Only the stream is copied back; on a parse error it is b""."""
+        m = _as_u8(msg)
+        flags = (FLAG_NDJSON if ndjson else 0) | (FLAG_COPY_STRINGS if copy_strings else 0)
+        n = C.c_size_t(0)
+        cap = 2 * m.size + 64  # tags + values are about 1.5x the input at most for typical JSON; else once more at the exact size
+        for _ in range(2):
+            out = np.empty(max(cap, 1), dtype=np.uint8)
+            rc = self.L.sj_parse_serialize(self.h, _addr(m) if m.size else None, m.size, flags, _addr(out), cap, C.byref(n))
+            if rc != ERR_CAPACITY:
+                break
+            cap = n.value
+        if rc in (ERR_STAGE1, ERR_STAGE2):
+            return rc, b""
+        if rc != OK:
+            raise SjError(rc)
+        return rc, out[:n.value].tobytes()
+
+    def serialize_device(self, tape, strings=None, message=None, out=None):
+        """Serializer.Serialize of a tape already on this context's device, arguments as marshal_device.  Returns (rc,
+        length of the stream, the uint8 tensor view holding it); SJ_ERR_CAPACITY when `out` is too small (the length is
+        still exact), SJ_ERR_ARGUMENT for a tape the reference's Serialize panics on."""
+        import torch
+        sp, sl = _ptr_len(strings)
+        mp, ml = _ptr_len(message)
+        tp, tl = _ptr_len(tape)
+        n = C.c_size_t(0)
+        if out is None:
+            rc = self.L.sj_serialize_device(self.h, mp, ml, tp, tl, sp, sl, None, 0, C.byref(n))
+            if rc not in (OK, ERR_CAPACITY):
+                return rc, n.value, None
+            out = torch.empty(max(n.value, 1), dtype=torch.uint8, device=tape.device)
+        rc = self.L.sj_serialize_device(self.h, mp, ml, tp, tl, sp, sl, out.data_ptr(), out.numel(), C.byref(n))
+        return rc, n.value, out[:n.value]
+
+    def deserialize_device(self, stream, tape=None, strings=None, message=None):
+        """Serializer.Deserialize (parsed_serialize.go:466) of a stream (uint8 tensor) on this context's device.  Writes
+        into `tape` (int64 tensor), `strings` and `message` (uint8 tensors), or new tensors when all three are None.
+        Returns (rc, (tape words, strings bytes, message bytes), (tape, strings, message) views).  rc is SJ_ERR_CAPACITY
+        when a buffer is too small (the sizes are still exact), SJ_ERR_UNSUPPORTED for S2 / zstd blocks and
+        SJ_ERR_ARGUMENT for a stream the device does not accept."""
+        import torch
+        ip, il = _ptr_len(stream)
+        tl, sl, ml = C.c_size_t(0), C.c_size_t(0), C.c_size_t(0)
+        dev = stream.device
+        if tape is None and strings is None and message is None:
+            rc = self.L.sj_deserialize_device(self.h, ip, il, None, 0, C.byref(tl), None, 0, C.byref(sl), None, 0, C.byref(ml))
+            if rc not in (OK, ERR_CAPACITY):
+                return rc, (tl.value, sl.value, ml.value), None
+            tape = torch.empty(max(tl.value, 1), dtype=torch.int64, device=dev)
+            strings = torch.empty(max(sl.value, 1), dtype=torch.uint8, device=dev)
+            message = torch.empty(max(ml.value, 1), dtype=torch.uint8, device=dev)
+
+        def buf(t):
+            return (t.data_ptr(), t.numel()) if t is not None else (None, 0)
+
+        (tp, tc), (sp, sc), (mp, mc) = buf(tape), buf(strings), buf(message)
+        rc = self.L.sj_deserialize_device(self.h, ip, il, tp, tc, C.byref(tl), sp, sc, C.byref(sl), mp, mc, C.byref(ml))
+        sizes = (tl.value, sl.value, ml.value)
+        if rc != OK:
+            return rc, sizes, None
+        return rc, sizes, (tape[:sizes[0]], strings[:sizes[1]], message[:sizes[2]])
+
+    def set_string_hash_bits(self, bits):
+        """test hook: keep only `bits` bits of the serializer's string hash (0 = all), to force collisions"""
+        rc = self.L.sj_test_set_string_hash_bits(self.h, int(bits))
+        if rc != OK:
+            raise SjError(rc)
+
     # ---- unit-test hooks (same method names as oracle.pyoracle.Oracle) -----------
     def block_masks(self, blocks, carries):
         """blocks: (n,64) uint8; carries: (n,4) uint64 -> (n,12) uint64 (see simdjson_b200.h)."""
@@ -248,6 +320,10 @@ class Context:
         return n.value
 
 
+def _ptr_len(t):
+    return (t.data_ptr(), t.numel()) if t is not None and t.numel() else (None, 0)
+
+
 _default_ctx = None
 
 
@@ -293,3 +369,35 @@ def Parse(b, reuse=None, copy_strings=True, ctx=None):
 def ParseND(b, reuse=None, copy_strings=True, ctx=None):
     """simdjson_amd64.go:82 ParseND: newline-delimited JSON."""
     return _parse(b, True, copy_strings, ctx)
+
+
+class Serializer:
+    """parsed_serialize.go:44 Serializer, on the default context's device.  Blocks are always uncompressed
+    (CompressNone), and strings are deduplicated exactly (first occurrence), so the stream does not depend on
+    copy_strings; the reference's Deserialize reads it."""
+
+    def __init__(self, ctx=None):
+        self.ctx = ctx
+
+    def Serialize(self, pj):
+        """the v3 stream of pj (a ParsedJson) as bytes"""
+        import torch
+        ctx = self.ctx or default_context()
+        tape = torch.from_numpy(np.ascontiguousarray(pj.Tape, dtype=np.uint64).view(np.int64)).cuda()
+        strs = torch.from_numpy(np.frombuffer(bytes(pj.Strings), dtype=np.uint8).copy()).cuda()
+        msg = torch.from_numpy(np.frombuffer(bytes(pj.Message), dtype=np.uint8).copy()).cuda()
+        rc, n, out = ctx.serialize_device(tape, strs, msg)
+        if rc != OK:
+            raise SjError(rc)
+        return out.cpu().numpy().tobytes()
+
+    def Deserialize(self, src):
+        """a ParsedJson from a v3 stream with uncompressed blocks (SJ_ERR_UNSUPPORTED for S2 / zstd blocks)"""
+        import torch
+        ctx = self.ctx or default_context()
+        d = torch.from_numpy(np.frombuffer(bytes(src), dtype=np.uint8).copy()).cuda()
+        rc, sizes, bufs = ctx.deserialize_device(d)
+        if rc != OK:
+            raise SjError(rc)
+        tape, strs, msg = (b.cpu().numpy() for b in bufs)
+        return ParsedJson(msg.tobytes(), tape.view(np.uint64).copy(), strs.tobytes())

@@ -10,7 +10,7 @@ import os
 _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.environ.get("SJ_B200_LIB") or os.path.join(os.path.dirname(_HERE), "libsimdjson_b200.so")  # override: another build, e.g. to compare two
 
-ERR_EXCHANGE, ERR_PEER, EXCHANGE_HANDLE_BYTES = 10, 11, 64
+ERR_EXCHANGE, ERR_PEER, ERR_UNSUPPORTED, EXCHANGE_HANDLE_BYTES = 10, 11, 12, 64
 FLAG_NDJSON = 1
 FLAG_COPY_STRINGS = 2
 OK, ERR_STAGE1, ERR_STAGE2, ERR_NO_DEVICE, ERR_CAPACITY, ERR_TOO_LARGE, ERR_ARGUMENT = range(7)
@@ -21,7 +21,8 @@ EXPORTS = [
     "sj_host_free", "sj_trim_space", "sj_bounds", "sj_parse", "sj_parse_device", "sj_gen_ndjson_device", "sj_parse_nd_sharded_count", "sj_parse_nd_sharded_emit", "sj_exchange_create", "sj_exchange_set_gap", "sj_exchange_set_timeout_ms", "sj_exchange_connect", "sj_exchange_connect_ptrs", "sj_exchange_local", "sj_exchange_bases", "sj_exchange_result", "sj_find_structural_indices", "sj_stage1_device",
     "sj_stage1_launch", "sj_ctx_sync", "sj_event_record", "sj_event_elapsed_ms", "sj_kernel_launches",
     "sj_test_block_masks", "sj_test_geometry", "sj_test_finalize", "sj_test_flatten_bits", "sj_test_parse_strings",
-    "sj_test_parse_numbers", "sj_count_where_device", "sj_parse_count_where", "sj_marshal_device", "sj_parse_marshal", "sj_stream_create", "sj_stream_destroy",
+    "sj_test_parse_numbers", "sj_count_where_device", "sj_parse_count_where", "sj_marshal_device", "sj_parse_marshal", "sj_serialize_device", "sj_parse_serialize",
+    "sj_deserialize_device", "sj_test_set_string_hash_bits", "sj_stream_create", "sj_stream_destroy",
     "sj_stream_write", "sj_stream_close_input", "sj_stream_next", "sj_stream_release",
 ]
 STREAM_END, STREAM_EMPTY, STREAM_BUSY = 7, 8, 9
@@ -136,6 +137,14 @@ def load():
     L.sj_marshal_device.argtypes = [vp, vp, sz, vp, sz, vp, sz, vp, sz, szp]
     L.sj_parse_marshal.restype = i32
     L.sj_parse_marshal.argtypes = [vp, vp, sz, u32, vp, sz, szp]
+    L.sj_serialize_device.restype = i32
+    L.sj_serialize_device.argtypes = [vp, vp, sz, vp, sz, vp, sz, vp, sz, szp]
+    L.sj_parse_serialize.restype = i32
+    L.sj_parse_serialize.argtypes = [vp, vp, sz, u32, vp, sz, szp]
+    L.sj_deserialize_device.restype = i32
+    L.sj_deserialize_device.argtypes = [vp, vp, sz, vp, sz, szp, vp, sz, szp, vp, sz, szp]
+    L.sj_test_set_string_hash_bits.restype = i32
+    L.sj_test_set_string_hash_bits.argtypes = [vp, i32]
     L.sj_stream_create.restype = i32
     L.sj_stream_create.argtypes = [i32, i32, sz, u32, C.POINTER(vp)]
     L.sj_stream_destroy.restype = None
