@@ -231,6 +231,12 @@ int sj_deserialize_device(sj_ctx* ctx, const uint8_t* d_in, size_t in_len, uint6
                           uint8_t* d_strings, size_t strings_cap, size_t* strings_len, uint8_t* d_msg, size_t msg_cap,
                           size_t* msg_len);
 int sj_test_set_string_hash_bits(sj_ctx* ctx, int bits);
+/*
+ * sj_test_stage2_internal: the internal-error word of the last parse through the streaming stage 2 (copy_strings):
+ * non-zero when the tape writer's counts of a slab differed from the ones stage 1 added up for it (the parse then
+ * returns SJ_ERR_STAGE2).  A defect of the library, never a verdict on the input: tests expect 0 on every input.
+ */
+int sj_test_stage2_internal(sj_ctx* ctx, uint32_t* word);
 
 /*
  * ParseNDStream (simdjson_amd64.go:116-215) inside the library: the caller pushes the bytes of an

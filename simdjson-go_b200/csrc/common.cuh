@@ -80,6 +80,28 @@ __device__ __forceinline__ uint32_t lanemask_lt() {
     return m;
 }
 
+// the warp of the portable stage-2 code (s2s_slab.h) on the device
+struct DevWarp {
+    __device__ __forceinline__ uint32_t lane() const { return threadIdx.x & 31; }
+    __device__ __forceinline__ uint32_t ballot(bool p) { return __ballot_sync(FULL, p); }
+    __device__ __forceinline__ bool any(bool p) { return __any_sync(FULL, p) != 0; }
+    __device__ __forceinline__ uint32_t shfl(uint32_t v, uint32_t src) { return __shfl_sync(FULL, v, (int)src); }
+    __device__ __forceinline__ uint32_t shfl_up(uint32_t v, int d) { return __shfl_up_sync(FULL, v, d); }
+    __device__ __forceinline__ uint32_t reduce_add(uint32_t v) { return __reduce_add_sync(FULL, v); }
+    __device__ __forceinline__ void sync() { __syncwarp(); }
+    __device__ __forceinline__ void atomic_and(uint32_t* p, uint32_t v) { atomicAnd(p, v); }
+    __device__ __forceinline__ void atomic_or(uint32_t* p, uint32_t v) { atomicOr(p, v); }
+    // LDGSTS: 16 bytes global -> shared without a register round trip; .ca keeps the line in L1 for the byte look-ups
+    __device__ __forceinline__ void async_copy16(void* dst, const void* src) {
+        asm volatile("cp.async.ca.shared.global [%0], [%1], 16;" ::"r"(smem_u32(dst)), "l"(src) : "memory");
+    }
+    __device__ __forceinline__ void async_commit() { asm volatile("cp.async.commit_group;" ::: "memory"); }
+    __device__ __forceinline__ void async_wait_prev() { asm volatile("cp.async.wait_group 1;" ::: "memory"); }
+    __device__ __forceinline__ void atomic_or_shared(uint32_t* p, uint32_t v) {
+        asm volatile("red.shared.or.b32 [%0], %1;" ::"r"(smem_u32(p)), "r"(v) : "memory");
+    }
+};
+
 #define SJ_CUDA_CHECK(expr)                                   \
     do {                                                      \
         cudaError_t _e = (expr);                              \

@@ -146,11 +146,19 @@ struct SlabAgg {
     uint32_t brk;    // brackets
     uint32_t rec;    // record boundaries (NDJSON roots - 1)
     int32_t depth;   // opens - closes
-    uint32_t ns;     // structurals (as stage 1 counts them: opening quotes, not closing ones)
+    uint32_t last;   // the bytes under the last three stage-1 structurals (byte 0: the last one), their count (0..3) in bits 24..25
     uint32_t num;    // numbers
     uint32_t trail;  // bit 31: the slab holds a real quote; bits 0..30: bytes behind the last one
 };
 constexpr uint32_t TRAIL_HASQ = 0x80000000u;
+
+// `last` of a in front of b: b's bytes are the later ones
+SJ_HD uint32_t last_combine(uint32_t a, uint32_t b) {
+    const uint32_t na = a >> 24, nb = b >> 24;
+    if (nb >= 3) return b;
+    const uint32_t n = na + nb < 3 ? na + nb : 3u;
+    return (((a << (8 * nb)) | b) & 0xffffffu) | (n << 24);
+}
 
 SJ_HD SlabAgg agg_zero() { return SlabAgg{0, 0, 0, 0, 0, 0, 0, 0}; }
 // a in front of b (not commutative in `trail`)
@@ -161,7 +169,7 @@ SJ_HD SlabAgg agg_combine(const SlabAgg& a, const SlabAgg& b) {
     r.brk = a.brk + b.brk;
     r.rec = a.rec + b.rec;
     r.depth = a.depth + b.depth;
-    r.ns = a.ns + b.ns;
+    r.last = last_combine(a.last, b.last);
     r.num = a.num + b.num;
     r.trail = (b.trail & TRAIL_HASQ) ? b.trail : ((a.trail & TRAIL_HASQ) | (((a.trail & ~TRAIL_HASQ) + b.trail) & ~TRAIL_HASQ));
     return r;
@@ -370,12 +378,10 @@ struct S2sParams {
     const uint8_t* msg;       // 16-byte aligned, readable up to round_up(len, 16)
     uint64_t len;
     uint32_t ndjson;
-    const uint32_t* idx;      // stage 1's structural positions (absolute): looked at only for what precedes a slab
-    uint32_t n_idx;
     const uint32_t* slabpar;  // per stage-1 tile: bit w = "inside a string" in front of slab w of the tile
     uint32_t slabs_per_tile;
     uint32_t nslabs;
-    SlabAgg* agg;             // [nslabs] K2p -> K2q
+    SlabAgg* agg;             // [nslabs] per-slab counts (stage 1's parse mode) -> K2q, and K2r's check of its own
     const SlabAgg* pre;       // [nslabs] exclusive prefix inside the slab's group of 1024 (K2q)
     const SlabAgg* grp_pre;   // [ngroups] exclusive prefix of the groups (K2q)
     // K2r outputs
@@ -389,6 +395,12 @@ struct S2sParams {
     uint32_t* rootpos;        // [records + 1] tape slot of each record's root-open word
     NumEntry* numlist;        // [numbers] in document order
     uint32_t* error;          // any stage-2 failure
+    uint32_t* internal;       // optional: K2r's view of a slab differs from stage 1's (an internal error, never a verdict on
+                              //   the input; the parse fails through `error` as well)
+    // optional: stage 1's structural positions (absolute), where the caller has them (the host emulation); K2r then also
+    // checks SlabAgg::last against the bytes under the last structurals in front of each slab.  The device parse has none.
+    const uint32_t* idx;
+    uint32_t n_idx;
     // NDJSON shards of ONE ParsedJson (simdjson_amd64.go:82-93): this parse's tape / Strings.B are the slices that
     // start at these offsets of the whole, so every index written INTO the tape is shifted by them
     // (root / scope pointers by tape_base, string offsets by str_base); both 0 for a stand-alone parse

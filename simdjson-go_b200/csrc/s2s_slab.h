@@ -1,7 +1,8 @@
 // s2s_slab.h -- streaming stage 2: what ONE WARP does with one 6 KiB slab, written once for the device (W = DevWarp,
 // stage2_stream.cuh) and for the host emulation (W = FiberWarp, tests/emu/s2s_emu.cpp).  See s2s_core.h for the idea.
 //
-//   s2s_slab<W, false>   K2p: counts of the slab -> SlabAgg
+//   s2s_slab<W, false>   counts of the slab -> SlabAgg (the emulator's counting pass; on the device stage 1's parse mode
+//                        counts, with step_events / agg_add_step below)
 //   s2s_slab<W, true>    K2r: tape words, Strings.B bytes, bracket records, number list, grammar masks
 //
 // W provides: lane(), ballot(bool), any(bool), shfl / shfl_up (uint32_t), reduce_add(uint32_t), sync(),
@@ -93,12 +94,20 @@ SJ_HD bool atom_ok_fast(const uint8_t* img, uint32_t o, uint32_t avail, uint32_t
 // shared-memory loads per digit in a kernel that is bound by dependent latencies.  Returns false when it does not apply; esc_decode (s2s_core.h) is the definition and
 // takes those cases -- including every digit quirk of parse_string_amd64.s:4-69, which is why only proper digits pass here.
 //   o: offset of the backslash in the image; avail: image bytes that are message bytes
-SJ_HD bool esc_u_fast(const uint8_t* img, uint32_t o, uint32_t avail, EscInfo& r) {
+//   at: where image offset o lives (SwzLayout: K2r's swizzled step image; FlatLayout: stage 1's tile buffer)
+struct SwzLayout {
+    SJ_HD uint32_t operator()(uint32_t o) const { return swz(o); }
+};
+struct FlatLayout {
+    SJ_HD uint32_t operator()(uint32_t o) const { return o; }
+};
+template <class A = SwzLayout>
+SJ_HD bool esc_u_fast(const uint8_t* img, uint32_t o, uint32_t avail, EscInfo& r, A at = A()) {
     if (o < 6 || o + 6 > avail) return false;
     const uint32_t a = (o - 6) & ~3u, sh = 8 * ((o - 6) & 3u);
     const uint32_t a3 = a + 12 < S2S_STEP_BYTES ? a + 12 : a + 8;  // (the fourth word only matters when sh != 0, and then it is inside)
-    const uint32_t w0 = *reinterpret_cast<const uint32_t*>(img + swz(a)), w1 = *reinterpret_cast<const uint32_t*>(img + swz(a + 4));
-    const uint32_t w2 = *reinterpret_cast<const uint32_t*>(img + swz(a + 8)), w3 = *reinterpret_cast<const uint32_t*>(img + swz(a3));
+    const uint32_t w0 = *reinterpret_cast<const uint32_t*>(img + at(a)), w1 = *reinterpret_cast<const uint32_t*>(img + at(a + 4));
+    const uint32_t w2 = *reinterpret_cast<const uint32_t*>(img + at(a + 8)), w3 = *reinterpret_cast<const uint32_t*>(img + at(a3));
     const uint32_t q0 = pi::funnel_r(w0, w1, sh), q1 = pi::funnel_r(w1, w2, sh), x = pi::funnel_r(w2, w3, sh);
     // q0 = bytes o-6 .. o-3, q1 = o-2 .. o+1, x = o+2 .. o+5 (the digits)
     if ((q1 >> 24) != 'u') return false;
@@ -191,6 +200,152 @@ SJ_HD uint32_t backslash_run_before_p(W& wp, const GlobalReader& g, uint64_t end
     }
 }
 
+// NDJSON: is the last structural in front of the slab a newline?  Outside a string that is "the last byte that is not a
+// blank, tab or CR is a newline" (every other byte is a structural of its own or belongs to a value that started behind
+// the last newline).  `peekc`: lane L holds the byte at slab_start - 1 - L (0x20 in front of the message).
+template <class W>
+SJ_HD uint32_t record_carry_in(W& wp, const GlobalReader& g, uint64_t slab_start, uint32_t peekc) {
+    const uint32_t lane = wp.lane();
+    for (uint64_t off = 0;; off += 32) {
+        const uint64_t back = off + lane + 1;
+        const uint32_t c = off == 0 ? peekc : (back <= slab_start ? g(slab_start - back) : 0x7fu);
+        const uint32_t solid = wp.ballot(!(c == 0x20 || c == 0x09 || c == 0x0d));
+        if (solid) return wp.shfl(c, pi::ctz64((uint64_t)solid)) == '\n' ? 1u : 0u;
+        if (back + 31 - lane >= slab_start) return 0;  // reached the start of the message: nothing but blanks
+    }
+}
+
+// What one 2 KiB step holds once its quote mask and its dropped escape bytes are known: stage 1's structurals, the
+// events of the tape, record starts, and the lane's counts.  The one definition of the counts: stage 1's parse mode
+// adds them up into the slab's SlabAgg, K2r turns the same masks into offsets.
+//   m: the classes of the lane's block (open, close, cc, ws, nl, numc, atomc are read); qm / qb: quote mask, real quotes;
+//   K: bytes of Strings.B; ppc / recc: the pseudo-structural and record carries, passed on to the next step
+struct StepEvents {
+    uint64_t brk;     // brackets outside strings
+    uint64_t st_out;  // brackets, commas, colons outside strings
+    uint64_t closeq;  // closing quotes
+    uint64_t V;       // value starts: atoms, numbers, garbage
+    uint64_t NLS;     // newlines outside strings (NDJSON)
+    uint64_t S;       // stage 1's structurals
+    uint64_t EV;      // the same with every string moved to its closing quote
+    uint64_t recst;   // record boundaries
+    uint32_t n_brk, n_open, n_num, n_rec, w_lane, k_lane, t_lane;
+    bool q_lane;
+};
+template <class W>
+SJ_HD StepEvents step_events(W& wp, const Class64& m, uint64_t qm, uint64_t qb, uint64_t K, uint32_t ndjson, uint32_t& ppc,
+                             uint32_t& recc) {
+    const uint32_t lane = wp.lane();
+    const uint32_t lt = (1u << lane) - 1u;
+    StepEvents e;
+    // finalize_structurals_amd64.s:19-36
+    e.brk = (m.open | m.close) & ~qm;
+    e.st_out = e.brk | (m.cc & ~qm);
+    e.closeq = qb & ~qm;
+    const uint64_t s0 = e.st_out | qb;
+    uint64_t pseudo;
+    {
+        const uint64_t pred = s0 | m.ws;
+        const uint32_t my_pp = (uint32_t)(pred >> 63);
+        const uint32_t up = wp.shfl_up(my_pp, 1);
+        const uint32_t pp_in = lane == 0 ? ppc : up;
+        ppc = wp.shfl(my_pp, 31);
+        pseudo = ((pred << 1) | pp_in) & ~m.ws & ~qm;
+    }
+    e.V = pseudo & ~s0;
+    e.NLS = ndjson ? (m.nl & ~qm) : 0ull;  // find_newline_delimiters_amd64.s:17-27
+    e.S = e.st_out | (qb & qm) | e.V | e.NLS;
+    e.EV = e.st_out | e.closeq | e.V | e.NLS;
+    // record boundaries: the first structural behind a run of newlines, if it is not a newline itself
+    // (stage2...go:200-221).  (T + ~S) carries from the byte behind each newline to the next structural.  They are
+    // counted where stage 1 sees that structural -- for a string at its OPENING quote -- so that the carry into
+    // a slab never depends on what lies in front of an open string.
+    e.recst = 0;
+    if (ndjson) {
+        const bool empty = e.S == 0;
+        const bool gen = !empty && ((e.NLS >> (63 - pi::clz64(e.S))) & 1ull);
+        const uint32_t Pm = wp.ballot(empty), G = wp.ballot(gen);
+        const uint32_t below = ~Pm & lt;
+        const uint32_t cin = below ? (G >> (31 - pi::clz32(below))) & 1u : recc;
+        const uint32_t nonp = ~Pm;
+        recc = nonp ? (G >> (31 - pi::clz32(nonp))) & 1u : recc;
+        const uint64_t T = (e.NLS << 1) | cin;
+        e.recst = (T + ~e.S) & e.S & ~e.NLS;
+    }
+    e.n_brk = pi::popc64(e.brk);
+    e.n_open = pi::popc64(m.open & ~qm);
+    const uint32_t n_str = pi::popc64(e.closeq), n_atom = pi::popc64(e.V & m.atomc);
+    e.n_num = pi::popc64(e.V & m.numc);
+    e.n_rec = pi::popc64(e.recst);
+    e.w_lane = e.n_brk + 2 * n_str + 2 * e.n_num + n_atom + 2 * e.n_rec;
+    e.k_lane = pi::popc64(K);
+    e.q_lane = qb != 0;
+    e.t_lane = e.q_lane ? pi::popc64(K & ~below64(64 - pi::clz64(qb))) : e.k_lane;  // bytes behind the lane's last quote
+    return e;
+}
+
+// The step's counts added to the slab's running totals.  `trail` / `hasq`: bytes behind the slab's last quote so far,
+// and whether it has one; SlabAgg::last is kept by the caller (agg_last_step).
+template <class W>
+SJ_HD void agg_add_step(W& wp, const StepEvents& e, SlabAgg& run, uint32_t& trail, uint32_t& hasq) {
+    const uint32_t lane = wp.lane();
+    run.w += wp.reduce_add(e.w_lane);
+    run.brk += wp.reduce_add(e.n_brk);
+    run.rec += wp.reduce_add(e.n_rec);
+    run.depth += (int32_t)wp.reduce_add(2 * e.n_open + 64 - e.n_brk) - 64 * 32;
+    run.num += wp.reduce_add(e.n_num);
+    const uint32_t k_step = wp.reduce_add(e.k_lane);
+    run.str += k_step;
+    const uint32_t Q = wp.ballot(e.q_lane);
+    if (Q) {
+        const uint32_t top = 31 - pi::clz32(Q);
+        trail = wp.shfl(e.t_lane, top) + wp.reduce_add(lane > top ? e.k_lane : 0u);
+        hasq = 1;
+    } else {
+        trail += k_step;
+    }
+}
+
+// SlabAgg::last of the step's structurals S, in front of which lie `last`; byte(o) = the step's byte at offset o
+template <class W, class B>
+SJ_HD uint32_t agg_last_step(W& wp, uint64_t S, uint32_t last, const B& byte) {
+    const uint32_t lane = wp.lane();
+    uint32_t v = 0, n = 0;
+    for (uint64_t r = S; r && n < 3; n++) {  // the lane's last three, the last one first
+        const uint32_t b = 63 - pi::clz64(r);
+        v |= byte(64 * lane + b) << (8 * n);
+        r &= ~(1ull << b);
+    }
+    v |= n << 24;
+    for (uint32_t d = 1; d < 32; d <<= 1) {  // lane 0 ends up with lanes 0..31 in order
+        const uint32_t o = wp.shfl(v, lane + d < 32 ? lane + d : lane);
+        if (lane + d < 32) v = last_combine(v, o);
+    }
+    return last_combine(last, wp.shfl(v, 0));
+}
+
+// Does SlabAgg::last in front of `slab` name the bytes under the last structurals of stage 1's index (p.idx) in front of
+// it -- the ones K2r takes as the events in front of the slab (par ? 2 : 1: inside a string the last structural is
+// that string's opening quote)?
+SJ_HD bool last_matches_index(const S2sParams& p, const GlobalReader& g, uint32_t slab, uint32_t last) {
+    const uint64_t slab_start = (uint64_t)slab * S2S_SLAB_BYTES;
+    uint32_t lo = 0, hi = p.n_idx;  // structurals in front of the slab
+    while (lo < hi) {
+        const uint32_t mid = lo + (hi - lo) / 2;
+        if (p.idx[mid] < slab_start)
+            lo = mid + 1;
+        else
+            hi = mid;
+    }
+    const uint32_t par = (p.slabpar[slab / p.slabs_per_tile] >> (slab % p.slabs_per_tile)) & 1u;
+    const uint32_t back = par ? 2u : 1u, n = last >> 24;
+    for (uint32_t k = back; k <= back + 1; k++) {
+        const uint32_t want = lo >= k ? g(p.idx[lo - k]) : 0u, got = n >= k ? (last >> (8 * (k - 1))) & 0xffu : 0u;
+        if (want != got) return false;
+    }
+    return true;
+}
+
 // Ask for the 2 KiB step that starts at message offset `first` into the image buffer `dst` (XOR-swizzled): whole
 // 16-byte chunks inside the message travel asynchronously (LDGSTS on the device), the chunk that holds the end of the
 // message and the chunks behind it are written directly, padded with spaces (find_structural_bits_amd64.s:167).
@@ -240,14 +395,14 @@ SJ_HD void s2s_slab(W& wp, const S2sParams& p, uint32_t slab, const S2sWarpMem& 
     bool have1 = false, have2 = false;
     if (EMIT) {
         run = agg_combine(p.grp_pre[slab >> 10], p.pre[slab]);
-        // from stage 1's index: inside a string the last structural is that string's opening quote, whose event
+        // from stage 1's last structurals: inside a string the last one is that string's opening quote, whose event
         // (the closing quote) is still to come
-        const uint32_t r = run.ns, back = par ? 2u : 1u;
+        const uint32_t r = run.last >> 24, back = par ? 2u : 1u;
         have1 = r >= back, have2 = r >= back + 1;
-        const uint32_t i1 = have1 ? p.idx[r - back] : 0u, i2 = have2 ? p.idx[r - back - 1] : 0u;
-        pc1 = have1 ? g(i1) : 0u;
-        pc2 = have2 ? g(i2) : 0u;
+        pc1 = have1 ? (run.last >> (8 * (back - 1))) & 0xffu : 0u;
+        pc2 = have2 ? (run.last >> (8 * back)) & 0xffu : 0u;
     }
+    const SlabAgg start = run;
     // the bytes in front of the slab (lanes 0..10: byte slab_start - 1 - lane), for an escape that straddles its start
     const uint32_t behind0 = (lane < 11 && slab_start > lane) ? g(slab_start - 1 - lane) : 0x20u;
     HeadInfo hd_next;
@@ -277,22 +432,7 @@ SJ_HD void s2s_slab(W& wp, const S2sParams& p, uint32_t slab, const S2sWarpMem& 
         const uint32_t is_st = prevc == '{' || prevc == '}' || prevc == '[' || prevc == ']' || prevc == ':' || prevc == ',';
         ppc = is_q | is_ws | (is_st & (par ^ 1u));
     }
-    // NDJSON: is the last structural in front of the slab a newline?  Outside a string that is "the last byte that is
-    // not a blank, tab or CR is a newline" (every other byte is a structural of its own or belongs to a value that
-    // started behind the last newline)
-    uint32_t recc = 0;
-    if (p.ndjson && !par && slab > 0) {
-        for (uint64_t off = 0;; off += 32) {
-            const uint64_t back = off + lane + 1;
-            const uint32_t c = off == 0 ? peekc : (back <= slab_start ? g(slab_start - back) : 0x7fu);
-            const uint32_t solid = wp.ballot(!(c == 0x20 || c == 0x09 || c == 0x0d));
-            if (solid) {
-                recc = wp.shfl(c, pi::ctz64((uint64_t)solid)) == '\n' ? 1u : 0u;
-                break;
-            }
-            if (back + 31 - lane >= slab_start) break;  // reached the start of the message: nothing but blanks
-        }
-    }
+    uint32_t recc = (p.ndjson && !par && slab > 0) ? record_carry_in(wp, g, slab_start, peekc) : 0u;
 
     // ---- running totals of the slab (K2p) / running prefixes (K2r) ----
     uint32_t trail = 0, hasq = 0;  // K2p: bytes behind the last quote so far
@@ -487,64 +627,15 @@ SJ_HD void s2s_slab(W& wp, const S2sParams& p, uint32_t slab, const S2sWarpMem& 
         }
 
         // ---------------- E: structurals (finalize_structurals_amd64.s:19-36), events, counts ----------------
-        const uint64_t brk_m = (m.open | m.close) & ~qm;
-        const uint64_t st_out = brk_m | (m.cc & ~qm);
-        const uint64_t closeq = qb & ~qm;
-        const uint64_t s0 = st_out | qb;
-        uint64_t pseudo;
-        {
-            const uint64_t pred = s0 | m.ws;
-            const uint32_t my_pp = (uint32_t)(pred >> 63);
-            const uint32_t up = wp.shfl_up(my_pp, 1);
-            const uint32_t pp_in = lane == 0 ? ppc : up;
-            ppc = wp.shfl(my_pp, 31);
-            pseudo = ((pred << 1) | pp_in) & ~m.ws & ~qm;
-        }
-        const uint64_t V = pseudo & ~s0;                        // value starts: atoms, numbers, garbage
-        const uint64_t NLS = p.ndjson ? (m.nl & ~qm) : 0ull;    // find_newline_delimiters_amd64.s:17-27
-        const uint64_t S = st_out | (qb & qm) | V | NLS;        // stage 1's structurals
-        const uint64_t EV = st_out | closeq | V | NLS;          // the same with every string moved to its closing quote
-        // record boundaries: the first structural behind a run of newlines, if it is not a newline itself
-        // (stage2...go:200-221).  (T + ~S) carries from the byte behind each newline to the next structural.  They are
-        // counted where stage 1 sees that structural -- for a string at its OPENING quote -- so that the carry into
-        // a slab never depends on what lies in front of an open string.
-        uint64_t recst = 0;
-        if (p.ndjson) {
-            const bool empty = S == 0;
-            const bool gen = !empty && ((NLS >> (63 - pi::clz64(S))) & 1ull);
-            const uint32_t Pm = wp.ballot(empty), G = wp.ballot(gen);
-            const uint32_t below = ~Pm & lt;
-            const uint32_t cin = below ? (G >> (31 - pi::clz32(below))) & 1u : recc;
-            const uint32_t nonp = ~Pm;
-            recc = nonp ? (G >> (31 - pi::clz32(nonp))) & 1u : recc;
-            const uint64_t T = (NLS << 1) | cin;
-            recst = (T + ~S) & S & ~NLS;
-        }
-        const uint32_t n_brk = pi::popc64(brk_m), n_open = pi::popc64(m.open & ~qm);
-        const uint32_t n_str = pi::popc64(closeq), n_num = pi::popc64(V & m.numc), n_atom = pi::popc64(V & m.atomc);
-        const uint32_t n_rec = pi::popc64(recst);
-        const uint32_t w_lane = n_brk + 2 * n_str + 2 * n_num + n_atom + 2 * n_rec;
-        const uint32_t k_lane = pi::popc64(K);
-        const bool q_lane = qb != 0;
-        const uint32_t t_lane = q_lane ? pi::popc64(K & ~below64(64 - pi::clz64(qb))) : k_lane;  // bytes behind the lane's last quote
+        const StepEvents ev = step_events(wp, m, qm, qb, K, p.ndjson, ppc, recc);
+        const uint64_t closeq = ev.closeq, V = ev.V, NLS = ev.NLS, EV = ev.EV, recst = ev.recst;
+        const uint32_t n_brk = ev.n_brk, n_open = ev.n_open, n_num = ev.n_num, n_rec = ev.n_rec;
+        const uint32_t w_lane = ev.w_lane, k_lane = ev.k_lane, t_lane = ev.t_lane;
+        const bool q_lane = ev.q_lane;
 
         if (!EMIT) {
-            run.w += wp.reduce_add(w_lane);
-            run.brk += wp.reduce_add(n_brk);
-            run.rec += wp.reduce_add(n_rec);
-            run.depth += (int32_t)wp.reduce_add(2 * n_open + 64 - n_brk) - 64 * 32;
-            run.ns += wp.reduce_add(pi::popc64(S));
-            run.num += wp.reduce_add(n_num);
-            const uint32_t k_step = wp.reduce_add(k_lane);
-            run.str += k_step;
-            const uint32_t Q = wp.ballot(q_lane);
-            if (Q) {
-                const uint32_t top = 31 - pi::clz32(Q);
-                trail = wp.shfl(t_lane, top) + wp.reduce_add(lane > top ? k_lane : 0u);
-                hasq = 1;
-            } else {
-                trail += k_step;
-            }
+            agg_add_step(wp, ev, run, trail, hasq);
+            run.last = agg_last_step(wp, ev.S, run.last, [&](uint32_t o) { return (uint32_t)sbase[swz(o)]; });
             continue;
         }
 
@@ -799,6 +890,18 @@ SJ_HD void s2s_slab(W& wp, const S2sParams& p, uint32_t slab, const S2sWarpMem& 
     }
 
     if (wp.any(err != 0) && lane == 0) wp.atomic_or(p.error, 1u);
+    if (EMIT && lane == 0) {  // the counts K2r went by against the ones stage 1 added up for the slab
+        const SlabAgg want = agg_combine(start, p.agg[slab]);
+        bool miscount = run.w != want.w || run.str != want.str || run.brk != want.brk || run.rec != want.rec ||
+                    run.depth != want.depth || run.num != want.num;
+#ifndef __CUDA_ARCH__  // (the device parse has no index; compiled there, the test costs K2r registers)
+        if (p.idx) miscount |= !last_matches_index(p, g, slab, start.last);
+#endif
+        if (miscount) {  // the tape is not to be trusted: the parse fails, and the internal word says why
+            wp.atomic_or(p.error, 1u);
+            if (p.internal) wp.atomic_or(p.internal, 1u);
+        }
+    }
     if (!EMIT && lane == 0) {
         run.trail = (hasq ? TRAIL_HASQ : 0u) | (trail & ~TRAIL_HASQ);
         p.agg[slab] = run;

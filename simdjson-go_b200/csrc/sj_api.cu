@@ -180,7 +180,10 @@ extern "C" int sj_ctx_create(int device, sj_ctx** out) {
                                            (int)S1_SMEM_BYTES));
         SJ_CUDA_CHECK(cudaFuncSetAttribute(stage1_flatten_kernel<true, true>, cudaFuncAttributeMaxDynamicSharedMemorySize,
                                            (int)S1_SMEM_BYTES));
-        SJ_CUDA_CHECK(cudaFuncSetAttribute(s2s_count_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)S2S_SMEM_COUNT));
+        SJ_CUDA_CHECK(cudaFuncSetAttribute(stage1_flatten_kernel<false, false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                           (int)S1_SMEM_BYTES));
+        SJ_CUDA_CHECK(cudaFuncSetAttribute(stage1_flatten_kernel<true, false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                           (int)S1_SMEM_BYTES));
         SJ_CUDA_CHECK(cudaFuncSetAttribute(s2s_emit_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)S2S_SMEM_EMIT));
         int per_sm = 0;
         SJ_CUDA_CHECK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, stage1_flatten_kernel<true, true>, S1_THREADS,
@@ -321,8 +324,10 @@ extern "C" int sj_kernel_launches(sj_ctx* c, uint64_t* count) {
 // ---------------------------------------------------------------------------------
 // stage 1
 // ---------------------------------------------------------------------------------
+// `agg` given: the parse mode of the streaming stage 2 -- no index (d_out / cap unused), per-slab counts into agg, an
+// invalid escape into *s2_error, the in-string bits of the slabs in the descriptor block (c->last_slabpar)
 static int launch_stage1(sj_ctx* c, const uint8_t* d_msg, size_t len, bool ndjson, bool deltas, uint32_t* d_out,
-                         size_t cap, uint32_t* d_bsmap = nullptr, bool want_slabpar = false) {
+                         size_t cap, uint32_t* d_bsmap = nullptr, SlabAgg* agg = nullptr, uint32_t* s2_error = nullptr) {
     if (len == 0 || len > SJ_MAX_MESSAGE) return SJ_ERR_TOO_LARGE;
     if ((reinterpret_cast<uintptr_t>(d_msg) & 15) != 0) return SJ_ERR_ARGUMENT;
     const int ntiles = (int)((len + S1_TILE_BYTES - 1) / S1_TILE_BYTES);
@@ -347,14 +352,17 @@ static int launch_stage1(sj_ctx* c, const uint8_t* d_msg, size_t len, bool ndjso
     p.result = &block->s1;
     p.ntiles = ntiles;
     p.bsmap = d_bsmap;
-    p.slabpar = want_slabpar ? reinterpret_cast<uint32_t*>(c->desc.as<uint8_t>() + off_slab) : nullptr;
+    p.slabpar = agg ? reinterpret_cast<uint32_t*>(c->desc.as<uint8_t>() + off_slab) : nullptr;
+    p.agg = agg;
+    p.s2_error = s2_error;
     c->last_slabpar = p.slabpar;
     int grid = ntiles;
     if (grid > c->s1_max_ctas) grid = c->s1_max_ctas;
     // cooperative launch: the static tile deal needs every CTA of the grid resident at once
     void* args[] = {&p};
-    const void* fn = ndjson ? (deltas ? (const void*)stage1_flatten_kernel<true, true> : (const void*)stage1_flatten_kernel<true, false>)
-                            : (deltas ? (const void*)stage1_flatten_kernel<false, true> : (const void*)stage1_flatten_kernel<false, false>);
+    const void* fn = agg ? (ndjson ? (const void*)stage1_flatten_kernel<true, false, true> : (const void*)stage1_flatten_kernel<false, false, true>)
+                     : ndjson ? (deltas ? (const void*)stage1_flatten_kernel<true, true> : (const void*)stage1_flatten_kernel<true, false>)
+                              : (deltas ? (const void*)stage1_flatten_kernel<false, true> : (const void*)stage1_flatten_kernel<false, false>);
     SJ_CUDA_CHECK(cudaLaunchCooperativeKernel(fn, dim3(grid), dim3(S1_THREADS), args, S1_SMEM_BYTES, c->stream));
     const int fgrid = (ntiles + 255) / 256;
     if (deltas)

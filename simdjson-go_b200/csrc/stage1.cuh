@@ -25,7 +25,7 @@
 #pragma once
 #include "bits.h"
 #include "common.cuh"
-#include "s2s_core.h"
+#include "s2s_slab.h"
 
 namespace sj {
 
@@ -659,6 +659,24 @@ struct Stage1Params {
     uint32_t* slabpar;   // optional: [ntiles] bit w = "inside a string" in front of slab w of the tile (handed to the streaming stage 2)
     Stage1Result* result;
     int ntiles;
+    // parse mode (the streaming stage 2 follows): no index; per slab the counts of stage 2 instead
+    SlabAgg* agg;        // [slabs] what s2s_slab<W, false> adds up for the slab
+    uint32_t* s2_error;  // an invalid escape (Stage2Result::error)
+};
+
+// message bytes for the escape decoder in parse mode: the slab's bytes from shared memory, others from global memory,
+// 0 beyond the end of the message
+struct SlabReader {
+    const uint8_t* src;
+    uint64_t start;
+    uint32_t win;  // message bytes the image holds
+    const uint8_t* msg;
+    uint64_t len;
+    __device__ __forceinline__ uint32_t operator()(uint64_t pos) const {
+        const uint64_t d = pos - start;
+        if (d < win) return src[d];
+        return pos < len ? msg[pos] : 0u;
+    }
 };
 
 __device__ __forceinline__ void load_block_words(const uint8_t* buf, uint32_t lane, uint32_t (&w)[16]) {
@@ -676,8 +694,11 @@ __device__ __forceinline__ void load_block_words(const uint8_t* buf, uint32_t la
     }
 }
 
-// bytes at or beyond `len` read as 0x20 (find_structural_bits_amd64.s:134-155)
-template <bool NDJSON, bool DELTAS>
+// bytes at or beyond `len` read as 0x20 (find_structural_bits_amd64.s:134-155).
+// PARSE: the streaming parse's stage 1.  No index is extracted or written (out / out_cap are not used); phase B adds
+// up, per slab, the counts stage 2 needs (SlabAgg: the same step_events / agg_add_step the emulator's counting pass
+// runs) from the masks it has at hand, with the slab's bytes still in shared memory.
+template <bool NDJSON, bool DELTAS, bool PARSE = false>
 __global__ void __launch_bounds__(S1_THREADS, S1_CTAS_PER_SM) stage1_flatten_kernel(const Stage1Params p) {
     extern __shared__ __align__(128) uint8_t smem[];
     // workers -> scan warp: quote parity, structural count, last structural (+1) of each slab
@@ -868,6 +889,7 @@ __global__ void __launch_bounds__(S1_THREADS, S1_CTAS_PER_SM) stage1_flatten_ker
         // ---------------- phase A: classify, escape analysis, slab quote parity ----------------
         uint64_t qb[S1_STEPS], st[S1_STEPS], ws[S1_STEPS], ct[S1_STEPS], nl[S1_STEPS], bsm[S1_STEPS], qmr[S1_STEPS];
         uint32_t slab_par = 0;
+        uint32_t cinbits = 0;  // PARSE: bit s = escape carry into the lane's block of step s
         uint32_t* const stage = reinterpret_cast<uint32_t*>(smem + (size_t)b * S1_TILE_BYTES + (size_t)warp * S1_SLAB_BYTES);
         const uint32_t pslab_pos = (uint32_t)(((uint64_t)prev_tile * S1_WARPS + warp) * S1_SLAB_BYTES);
 #pragma unroll
@@ -903,6 +925,7 @@ __global__ void __launch_bounds__(S1_THREADS, S1_CTAS_PER_SM) stage1_flatten_ker
                     uint32_t nonpass = ~A;
                     bs_carry = nonpass ? (F >> (31 - __clz(nonpass))) & 1 : bs_carry;
                     odd_ends = odd_backslash_ends(bs, cin, nullptr);
+                    if (PARSE) cinbits |= cin << s;
                 }
                 qb[s] &= ~odd_ends;
                 // quote mask relative to the start of the slab (find_quote_mask_and_bits_amd64.s:49-66); the
@@ -928,7 +951,7 @@ __global__ void __launch_bounds__(S1_THREADS, S1_CTAS_PER_SM) stage1_flatten_ker
         // it, in phase A above)
         uint32_t staged = 0;  // entries staged (warp-uniform)
         uint32_t dense = 0;   // more than one structural per 4 bytes: the slab does not fit its own staging area
-        if (have_prev) {
+        if (!PARSE && have_prev) {
             __syncwarp();
 #pragma unroll
             for (int s = 0; s < S1_STEPS; s++) {
@@ -944,7 +967,7 @@ __global__ void __launch_bounds__(S1_THREADS, S1_CTAS_PER_SM) stage1_flatten_ker
         __syncwarp();            // staged positions of all lanes are visible
 
         // ---------------- copy-out of the previous tile's staged structurals ----------------
-        if (have_prev) {
+        if (!PARSE && have_prev) {
             // deltas: the first structural of a tile is written as pos + 1 here and rebased on the
             // previous tile's last structural by stage1_finish_kernel
             uint32_t prev_last = s_wlast[warp] - 1;  // 0xffffffff when nothing precedes inside the tile
@@ -975,6 +998,85 @@ __global__ void __launch_bounds__(S1_THREADS, S1_CTAS_PER_SM) stage1_flatten_ker
         uint32_t err = 0;
         uint32_t slab_count = 0;
         const uint64_t flip = par_in ? ~0ull : 0ull;
+        if constexpr (PARSE) {
+            // stage 2's counts of the slab, as s2s_slab<W, false> adds them up (the carries into the slab are the ones
+            // worked out above, or from the bytes in front of it as it does)
+            DevWarp wp;
+            const GlobalReader g{p.msg, p.len};
+            const SlabReader rd{buf, slab_start, active ? (uint32_t)min((uint64_t)S1_SLAB_BYTES, p.len - slab_start) : 0u, p.msg, p.len};
+            SlabAgg run = agg_zero();
+            uint32_t trail = 0, hasq = 0, s2err = 0, hd_drop = 0;
+            uint32_t ppc = pp_carry;
+            uint32_t recc = (NDJSON && active && !par_in && slab > 0) ? record_carry_in(wp, g, slab_start, peekc) : 0u;
+#pragma unroll
+            for (int s = 0; s < S1_STEPS; s++) {
+                const uint64_t qm = qmr[s] ^ flip;
+                if (ct[s] & qm) err = 1;  // find_quote_mask_and_bits_amd64.s:69-80
+                const uint64_t step_start = slab_start + (uint64_t)s * S1_STEP_BYTES;
+                uint64_t fin = 0;
+                if (active && step_start < p.len) {  // warp-uniform
+                    uint32_t w[16];
+                    load_block_words(buf + s * S1_STEP_BYTES, lane, w);
+                    const Class64 c = classify_block2(w);
+                    Class64 m;
+                    m.open = rotl16x((uint32_t)c.open, (uint32_t)(c.open >> 32), rsel);
+                    m.close = rotl16x((uint32_t)c.close, (uint32_t)(c.close >> 32), rsel);
+                    m.cc = rotl16x((uint32_t)c.cc, (uint32_t)(c.cc >> 32), rsel);
+                    m.numc = rotl16x((uint32_t)c.numc, (uint32_t)(c.numc >> 32), rsel);
+                    m.atomc = rotl16x((uint32_t)c.atomc, (uint32_t)(c.atomc >> 32), rsel);
+                    m.ws = ws[s];
+                    m.nl = nl[s];
+                    // escapes inside strings -> the bytes they drop from Strings.B; what an escape that starts in front
+                    // of the step leaves behind its start: head_info at the slab start, the previous step's last lane
+                    // inside the slab
+                    const uint64_t bsr = rotl16x((uint32_t)c.bs, (uint32_t)(c.bs >> 32), rsel);
+                    const uint64_t Ein = escape_starts(bsr, (cinbits >> s) & 1u) & qm;
+                    if (s == 0) {
+                        const HeadInfo hd = head_info(wp, g, step_start, par_in != 0, peekc);
+                        hd_drop = hd.drop;
+                        s2err |= hd.bad;
+                    }
+                    uint64_t D = 0;
+                    uint32_t next_drop = 0;
+                    if (__any_sync(FULL, Ein != 0)) {
+                        uint32_t spill = 0;  // dropped bytes of the lane's escapes that lie in the next block
+                        const uint64_t bp = step_start + 64 * lane;
+                        for (uint64_t r = Ein; r; r &= r - 1) {
+                            const uint32_t j = (uint32_t)__ffsll((long long)r) - 1;
+                            EscInfo ei;
+                            if (!esc_u_fast(buf + s * S1_STEP_BYTES, 64 * lane + j, (uint32_t)min((uint64_t)S1_STEP_BYTES, p.len - step_start), ei,
+                                            FlatLayout()))
+                                ei = esc_decode(rd, g, bp + j);
+                            if (ei.second) continue;
+                            if (!ei.valid) {
+                                s2err = 1;
+                                continue;
+                            }
+                            const uint32_t hi = j + ei.c - ei.n;  // all c source bytes are dropped except the last n
+                            D |= range64(j, hi < 64 ? hi : 64);
+                            if (hi > 64) spill |= (uint32_t)below64(hi - 64);
+                        }
+                        const uint32_t up = __shfl_up_sync(FULL, spill, 1);
+                        if (lane) D |= up;
+                        next_drop = __shfl_sync(FULL, spill, 31);
+                    }
+                    if (lane == 0) D |= hd_drop;
+                    hd_drop = next_drop;
+                    const uint64_t K = qm & ~qb[s] & ~D;
+                    const StepEvents e = step_events(wp, m, qm, qb[s], K, NDJSON ? 1u : 0u, ppc, recc);
+                    agg_add_step(wp, e, run, trail, hasq);
+                    run.last = agg_last_step(wp, e.S, run.last, [&](uint32_t o) { return (uint32_t)buf[s * S1_STEP_BYTES + o]; });
+                    fin = e.S;
+                }
+                S_prev[s] = fin;
+                slab_count += __popcll(fin);
+            }
+            if (__any_sync(FULL, s2err) && lane == 0) atomicOr(p.s2_error, 1u);
+            if (active && lane == 0) {
+                run.trail = (hasq ? TRAIL_HASQ : 0u) | (trail & ~TRAIL_HASQ);
+                p.agg[slab] = run;
+            }
+        } else {
 #pragma unroll
         for (int s = 0; s < S1_STEPS; s++) {
             const uint64_t qm = qmr[s] ^ flip;
@@ -991,6 +1093,7 @@ __global__ void __launch_bounds__(S1_THREADS, S1_CTAS_PER_SM) stage1_flatten_ker
             if (!active) fin = 0;
             S_prev[s] = fin;  // flattened in the next iteration
             slab_count += __popcll(fin);
+        }
         }
 #pragma unroll
         for (int d = 16; d > 0; d >>= 1) slab_count += __shfl_xor_sync(FULL, slab_count, d);

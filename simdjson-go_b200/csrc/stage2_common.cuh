@@ -24,6 +24,7 @@ struct Stage2Result {
     uint32_t overflow;     // tape / string capacity exceeded
     uint32_t n_numbers;    // structurals that start a number (K2a)
     uint32_t num_fill;     // fill pointer of the number list (K2g)
+    uint32_t internal;     // streaming stage 2: K2r's counts of a slab differ from stage 1's (a defect of the library, not of the input)
 };
 
 __device__ __forceinline__ SlabAgg agg_shfl_up(const SlabAgg& a, int d) {
@@ -33,7 +34,7 @@ __device__ __forceinline__ SlabAgg agg_shfl_up(const SlabAgg& a, int d) {
     r.brk = __shfl_up_sync(FULL, a.brk, d);
     r.rec = __shfl_up_sync(FULL, a.rec, d);
     r.depth = __shfl_up_sync(FULL, a.depth, d);
-    r.ns = __shfl_up_sync(FULL, a.ns, d);
+    r.last = __shfl_up_sync(FULL, a.last, d);
     r.num = __shfl_up_sync(FULL, a.num, d);
     r.trail = __shfl_up_sync(FULL, a.trail, d);
     return r;

@@ -1,7 +1,8 @@
 // stage2_stream.cuh -- the streaming stage 2 on the device: kernels around the portable core (s2s_core.h, s2s_slab.h).
 //
-//   K2p s2s_count      one warp per 6 KiB slab: per-slab aggregate (tape words, string bytes, brackets, depth, records,
-//                      structurals, numbers, bytes behind the last quote)
+//   K1  stage1_flatten_kernel<., ., true> (stage1.cuh), the parse mode of stage 1: besides the in-string state of every
+//                      slab, per-slab aggregate (tape words, string bytes, brackets, depth, records, the bytes under the
+//                      last stage-1 structurals, numbers, bytes behind the last quote)
 //   K2q scan_*_kernel<SlabAgg> (stage2_common.cuh)   exclusive scan of the aggregates (groups of 1024 + their
 //                      totals), grand totals -> Stage2Result
 //   K2r s2s_emit       the same analysis again, now with every offset known: tape words, Strings.B bytes (compacted in
@@ -31,35 +32,11 @@ static_assert(S1_WARPS <= 32, "one bit per slab of a tile");
 constexpr int S2S_WARPS = 8;  // slabs per CTA
 constexpr int S2S_THREADS = S2S_WARPS * 32;
 constexpr uint32_t S2S_SSTAGE_PAD = (S2S_SSTAGE_BYTES + 15u) & ~15u;
-constexpr uint32_t S2S_WARP_SMEM_COUNT = S2S_IMAGE_BYTES + S2S_ESC_SCRATCH;
 static_assert(S2S_TSTAGE_WORDS * 8 >= S2S_ESC_SCRATCH, "K2r decodes escapes in the tape-staging area");
 constexpr uint32_t S2S_WARP_SMEM_EMIT = S2S_IMAGE_BYTES + S2S_SSTAGE_PAD + S2S_TSTAGE_WORDS * 8;
-constexpr size_t S2S_SMEM_COUNT = (size_t)S2S_WARPS * S2S_WARP_SMEM_COUNT;
 constexpr size_t S2S_SMEM_EMIT = (size_t)S2S_WARPS * S2S_WARP_SMEM_EMIT;
 // resident blocks per SM the register allocation must allow; also the persistent grids' blocks per SM
 constexpr int S2S_EMIT_MIN_BLOCKS = 2;
-constexpr int S2S_COUNT_MIN_BLOCKS = 3;
-
-struct DevWarp {
-    __device__ __forceinline__ uint32_t lane() const { return threadIdx.x & 31; }
-    __device__ __forceinline__ uint32_t ballot(bool p) { return __ballot_sync(FULL, p); }
-    __device__ __forceinline__ bool any(bool p) { return __any_sync(FULL, p) != 0; }
-    __device__ __forceinline__ uint32_t shfl(uint32_t v, uint32_t src) { return __shfl_sync(FULL, v, (int)src); }
-    __device__ __forceinline__ uint32_t shfl_up(uint32_t v, int d) { return __shfl_up_sync(FULL, v, d); }
-    __device__ __forceinline__ uint32_t reduce_add(uint32_t v) { return __reduce_add_sync(FULL, v); }
-    __device__ __forceinline__ void sync() { __syncwarp(); }
-    __device__ __forceinline__ void atomic_and(uint32_t* p, uint32_t v) { atomicAnd(p, v); }
-    __device__ __forceinline__ void atomic_or(uint32_t* p, uint32_t v) { atomicOr(p, v); }
-    // LDGSTS: 16 bytes global -> shared without a register round trip; .ca keeps the line in L1 for the byte look-ups
-    __device__ __forceinline__ void async_copy16(void* dst, const void* src) {
-        asm volatile("cp.async.ca.shared.global [%0], [%1], 16;" ::"r"(smem_u32(dst)), "l"(src) : "memory");
-    }
-    __device__ __forceinline__ void async_commit() { asm volatile("cp.async.commit_group;" ::: "memory"); }
-    __device__ __forceinline__ void async_wait_prev() { asm volatile("cp.async.wait_group 1;" ::: "memory"); }
-    __device__ __forceinline__ void atomic_or_shared(uint32_t* p, uint32_t v) {
-        asm volatile("red.shared.or.b32 [%0], %1;" ::"r"(smem_u32(p)), "r"(v) : "memory");
-    }
-};
 
 // character / transition / compaction tables of a CTA (shared memory)
 struct S2sTables {
@@ -74,24 +51,6 @@ __device__ __forceinline__ void s2s_fill_tables(S2sTables& t) {
         t.oktab[i] = (p < 15 && c < 15) ? (uint8_t)transition_mask(p, c) : (uint8_t)0;
     }
     if (threadIdx.x < 16) t.cmptab[threadIdx.x] = compress_sel(threadIdx.x) | ((uint32_t)__popc(threadIdx.x) << 16);
-}
-
-__global__ void __launch_bounds__(S2S_THREADS, S2S_COUNT_MIN_BLOCKS) s2s_count_kernel(const S2sParams p) {
-    extern __shared__ __align__(128) uint8_t s2s_smem[];
-    __shared__ S2sTables tabs;
-    s2s_fill_tables(tabs);
-    __syncthreads();
-    const uint32_t warp = threadIdx.x >> 5;
-    S2sWarpMem sm;
-    sm.src = s2s_smem + (size_t)warp * S2S_WARP_SMEM_COUNT;
-    sm.sstage = nullptr;
-    sm.tstage = nullptr;
-    sm.esc = sm.src + S2S_IMAGE_BYTES;
-    sm.ctab = tabs.ctab;
-    sm.oktab = tabs.oktab;
-    sm.cmptab = tabs.cmptab;
-    DevWarp wp;
-    s2s_warp_loop<DevWarp, false>(wp, p, blockIdx.x * S2S_WARPS + warp, gridDim.x * S2S_WARPS, sm);
 }
 
 __global__ void __launch_bounds__(S2S_THREADS, S2S_EMIT_MIN_BLOCKS) s2s_emit_kernel(const S2sParams p) {

@@ -11,5 +11,5 @@ MIB=${2:-64}
 mkdir -p $O
 B="python tools/config_bench.py $MIB $IN"
 timeout 280 ncu --set full --import-source on --clock-control none -k regex:s2s_emit_kernel -s 3 -c 1 -o $O/k2r_$IN -f $B > $O/ncu_k2r_$IN.log 2>&1
-timeout 280 ncu --set full --import-source on --clock-control none -k regex:s2s_count_kernel -s 3 -c 1 -o $O/k2p_$IN -f $B > $O/ncu_k2p_$IN.log 2>&1
+timeout 280 ncu --set full --import-source on --clock-control none -k 'regex:stage1_flatten_kernel<[a-z]+, false, true>' -s 3 -c 1 -o $O/k1parse_$IN -f $B > $O/ncu_k1parse_$IN.log 2>&1
 ls -la $O/*.ncu-rep
