@@ -134,8 +134,15 @@ constexpr uint32_t S2S_SLAB_BYTES = S2S_STEPS * S2S_STEP_BYTES;      // == S1_SL
 constexpr uint32_t S2S_IMAGE_BYTES = 2 * S2S_STEP_BYTES;              // two image buffers: the step at hand and the next one in flight
 constexpr uint32_t S2S_SSTAGE_BYTES = S2S_STEP_BYTES + 32;           // compacted string bytes of one step (+ alignment shift)
 // K2r's tape-staging area (8-byte words), which holds the escape scratch: more than the escapes need, and its size is
-// part of K2r's shared memory per block, so it sets K2r's occupancy
+// part of K2r's shared memory per block, so it sets K2r's occupancy.  A step whose tape words (plus the destination's
+// phase inside its 32-byte sector) fit is staged here and copied out in whole sectors; a denser one stores directly.
 constexpr uint32_t S2S_TSTAGE_WORDS = 640;
+// lists of a staged step's brackets and record starts, kept in the string staging area once Strings.B is out; a step
+// with more of them leaves all its links to K2e / K2f
+constexpr uint32_t S2S_LINK_BRK_CAP = 384, S2S_LINK_REC_CAP = 128;
+constexpr uint32_t S2S_LINK_SCAN = 64;  // brackets a close looks back for its partner inside the step
+// brk_kind bit: K2r has written both cross-links of this close (its partner lies in the same step), K2e skips them
+constexpr uint8_t BRK_LINKED = 0x80;
 
 // per-slab aggregate (K2p) / exclusive prefix (K2q).  `trail`: string-buffer bytes behind the last real quote of
 // the slab (all of them if the slab holds no quote) -- scanned with the segmented operator below it gives, for a
@@ -389,10 +396,13 @@ struct S2sParams {
     uint8_t* strings;
     uint32_t* brk_tp;         // [nb] tape slot of bracket k
     int32_t* brk_depth;       // [nb] depth in front of it
-    uint8_t* brk_kind;        // [nb] T_OBJ_OPEN .. T_ARR_CLOSE
+    uint8_t* brk_kind;        // [nb] T_OBJ_OPEN .. T_ARR_CLOSE, | BRK_LINKED on a close K2r has cross-linked
     uint32_t* segmask;        // [(nb + 1 + 3) / 4] one byte per bracket-to-bracket segment, preset to 0xff: bit ctx = every
                               //   structural of the segment is allowed inside a container of kind ctx
     uint32_t* rootpos;        // [records + 1] tape slot of each record's root-open word
+    uint32_t* rootlink;       // [(records + 1 + 31) / 32] preset to all ones; bit r cleared: K2r has written record r's two
+                              //   root words (its open and the next record's open lie in one staged step), K2f skips them.
+                              //   Optional: without it K2r writes no root words and K2f writes them all
     NumEntry* numlist;        // [numbers] in document order
     uint32_t* error;          // any stage-2 failure
     uint32_t* internal;       // optional: K2r's view of a slab differs from stage 1's (an internal error, never a verdict on

@@ -737,8 +737,26 @@ SJ_HD void s2s_slab(W& wp, const S2sParams& p, uint32_t slab, const S2sWarpMem& 
             }
         }
 
-        // ---------------- the lane's events, in order (tape words go straight to global memory) ----------------
+        // ---------------- the lane's events, in order ----------------
+        // The step's tape words [slot0, slot0 + w_step) go to the tape-staging area at the destination's 32-byte phase
+        // and out in whole sectors behind the loops; scattered 8-byte stores straight to the tape would each land on a
+        // sector of their own.  A step that does not fit (dense brackets: up to ~2048 words) stores directly.
         const uint32_t slot0 = 1 + run.w;                // tape slot of the step's first word (slot 0: the first root word)
+        const uint32_t ph = (uint32_t)(reinterpret_cast<uintptr_t>(p.tape + slot0) >> 3) & 3u;  // (the tape is 8-byte aligned)
+        const uint32_t sslot = slot0 - ph;               // slot of staging word 0 (modulo 2^32: it may lie in front of slot 0)
+        const bool staged = ph + w_step <= S2S_TSTAGE_WORDS;  // warp-uniform, as are the two below
+        // brackets and record starts of a staged step are listed in the string staging area, so that the pairs with both
+        // ends in the step are linked here (K2e and K2f then skip them)
+        const bool link_b = staged && b_step != 0 && b_step <= S2S_LINK_BRK_CAP;
+        const bool link_r = staged && r_step >= 2 && r_step <= S2S_LINK_REC_CAP && p.rootlink != nullptr;
+        uint32_t* const lst = reinterpret_cast<uint32_t*>(sm.sstage);  // [0, BRK_CAP): brackets, then record starts
+        if (k_step && (link_b || link_r)) wp.sync();      // (Strings.B's copy-out has read the string staging area)
+        auto put = [&](uint32_t slot, uint64_t v) {
+            if (staged)
+                sm.tstage[slot - sslot] = v;
+            else
+                p.tape[slot] = v;
+        };
         {
             // refined type of the last event in front of the lane
             const uint32_t nev = pi::popc64(EV);
@@ -809,11 +827,13 @@ SJ_HD void s2s_slab(W& wp, const S2sParams& p, uint32_t slab, const S2sWarpMem& 
                 const uint32_t num = (uint32_t)(NUM >> (32 * h)), atm = (uint32_t)(ATOM >> (32 * h));
                 const uint32_t bdr = (uint32_t)(BADR >> (32 * h)), bdo = (uint32_t)(BADO >> (32 * h)), bda = (uint32_t)(BADA >> (32 * h));
                 const uint64_t half_pos = block_pos + 32 * h;
-                // record boundaries (root close + root open: the words themselves are written by K2f)
+                // record boundaries (root close + root open: the words themselves are written by K2f, or below)
                 for (uint32_t mm = rs; mm; mm &= mm - 1) {
                     const uint32_t lo = (1u << pi::ctz32(mm)) - 1u;
                     const uint32_t below = pi::popc32(rs & lo);
-                    p.rootpos[rec_b + below + 1] = words_b + pi::popc32(w1 & lo) + 2 * (pi::popc32(w2 & lo) + below) + 1;
+                    const uint32_t open = words_b + pi::popc32(w1 & lo) + 2 * (pi::popc32(w2 & lo) + below) + 1;
+                    p.rootpos[rec_b + below + 1] = open;
+                    if (link_r) lst[S2S_LINK_BRK_CAP + rec_b - run.rec + below] = open;
                 }
                 // brackets: records for the scope matching, the tape word, the grammar verdict of the segment they end
                 {
@@ -823,10 +843,15 @@ SJ_HD void s2s_slab(W& wp, const S2sParams& p, uint32_t slab, const S2sWarpMem& 
                         const uint32_t slot = words_b + pi::popc32(w1 & lo) + 2 * (pi::popc32(w2 & lo) + pi::popc32(rs & upto));
                         const uint32_t kb = kb_b + pi::popc32(brk & lo);
                         const bool curly = (cur & bit) != 0, opening = (opn & bit) != 0;
+                        const int32_t dep = depth_b + (int32_t)pi::popc32(opn & lo) - (int32_t)pi::popc32(brk & ~opn & lo);
+                        const uint32_t kind = opening ? (curly ? T_OBJ_OPEN : T_ARR_OPEN) : (curly ? T_OBJ_CLOSE : T_ARR_CLOSE);
                         p.brk_tp[kb] = slot;
-                        p.brk_depth[kb] = depth_b + (int32_t)pi::popc32(opn & lo) - (int32_t)pi::popc32(brk & ~opn & lo);
-                        p.brk_kind[kb] = (uint8_t)(opening ? (curly ? T_OBJ_OPEN : T_ARR_OPEN) : (curly ? T_OBJ_CLOSE : T_ARR_CLOSE));
-                        p.tape[slot] = (uint64_t)((opening ? 0x5bu : 0x5du) | (curly ? 0x20u : 0u)) << 56;  // payload cross-linked after the scope matching
+                        p.brk_depth[kb] = dep;
+                        if (link_b)  // staging index (10 bits) | kind (3) | depth in front relative to the step's, + 4096 (13)
+                            lst[kb - run.brk] = (slot - sslot) | (kind << 10) | ((uint32_t)(dep - run.depth + 4096) << 13);
+                        else
+                            p.brk_kind[kb] = (uint8_t)kind;
+                        put(slot, (uint64_t)((opening ? 0x5bu : 0x5du) | (curly ? 0x20u : 0u)) << 56);  // payload: cross-linked below or by K2e
                         const uint32_t seg = upto & ~prevm;
                         const uint32_t bad = segbad | ((bdr & seg) ? 1u : 0u) | ((bdo & seg) ? 2u : 0u) | ((bda & seg) ? 4u : 0u);
                         if (bad) wp.atomic_and(p.segmask + (kb >> 2), ~(bad << (8 * (kb & 3))));
@@ -843,8 +868,8 @@ SJ_HD void s2s_slab(W& wp, const S2sParams& p, uint32_t slab, const S2sWarpMem& 
                     const uint32_t kbelow = pi::popc32(kk & lo);
                     const uint32_t lower = qq & lo;  // the opening quote is the highest quote below, if it is in this half
                     const uint32_t dl = lower ? pi::popc32(kk & lo & ~((1u << (31 - pi::clz32(lower))) - 1u)) : pre_dl + kbelow;
-                    p.tape[slot] = ((uint64_t)'"' << 56) | (STRINGBUFBIT + out_str_base + (uint64_t)(lane_str + rank_b + kbelow - dl));
-                    p.tape[slot + 1] = dl;
+                    put(slot, ((uint64_t)'"' << 56) | (STRINGBUFBIT + out_str_base + (uint64_t)(lane_str + rank_b + kbelow - dl)));
+                    put(slot + 1, dl);
                 }
                 // numbers: parsed by K2h from the list
                 for (uint32_t mm = num; mm; mm &= mm - 1) {
@@ -865,7 +890,7 @@ SJ_HD void s2s_slab(W& wp, const S2sParams& p, uint32_t slab, const S2sWarpMem& 
                         ok = atom_ok_p(rd, half_pos + j, p.len, sm.ctab[ch]);
                     }
                     if (!ok) err = 1;
-                    p.tape[slot] = (uint64_t)ch << 56;
+                    put(slot, (uint64_t)ch << 56);
                 }
                 // totals of the half
                 const uint32_t nk = pi::popc32(kk), nopn = pi::popc32(opn), nbr = pi::popc32(brk);
@@ -880,7 +905,67 @@ SJ_HD void s2s_slab(W& wp, const S2sParams& p, uint32_t slab, const S2sWarpMem& 
             // the segment behind the lane's last bracket goes on in the next lanes
             if (segbad) wp.atomic_and(p.segmask + (kb_b >> 2), ~(segbad << (8 * (kb_b & 3))));
         }
-        wp.sync();  // the string staging area and the escape scratch are reused by the next step
+        if (staged) {
+            wp.sync();
+            if (link_b || link_r) {
+                const uint64_t tb = s2s_tape_base(p);
+                // a close whose partner -- the nearest bracket in front of it with a smaller depth in front, K2d's rule;
+                // none for a close at the top level -- lies in the step gets both cross-links (K2e's words) and BRK_LINKED
+                for (uint32_t i = lane; link_b && i < b_step; i += 32) {
+                    const uint32_t e = lst[i], kind = (e >> 10) & 7u, t = e >> 13;
+                    uint32_t linked = 0;
+                    if ((kind == T_OBJ_CLOSE || kind == T_ARR_CLOSE) && run.depth + (int32_t)t - 4096 > 0) {
+                        const uint32_t stop = i > S2S_LINK_SCAN ? i - S2S_LINK_SCAN : 0u;
+                        for (uint32_t j = i; j > stop;) {
+                            const uint32_t f = lst[j - 1], d = f >> 13;
+                            if (d < t) {
+                                const uint32_t o = f & 0x3ffu, c = e & 0x3ffu;  // staging indices of the pair
+                                const bool curly = kind == T_OBJ_CLOSE;
+                                sm.tstage[o] = ((uint64_t)(curly ? '{' : '[') << 56) | (tb + (uint32_t)(sslot + c + 1));
+                                sm.tstage[c] = ((uint64_t)(curly ? '}' : ']') << 56) | (tb + (uint32_t)(sslot + o));
+                                linked = BRK_LINKED;
+                                break;
+                            }
+                            // the depth moves by one per bracket: the d - t brackets in front of this one are no shallower
+                            const uint32_t skip = 1 + d - t;
+                            j = j > stop + skip ? j - skip : stop;
+                        }
+                    }
+                    p.brk_kind[run.brk + i] = (uint8_t)(kind | linked);
+                }
+                // records r = run.rec + 1 + i whose open (record start i of the step) and whose close (in front of record
+                // start i + 1) both lie in the step: both root words (K2f's), and their rootlink bits cleared
+                if (link_r) {
+                    const uint64_t R = (uint64_t)'r' << 56;
+                    const uint32_t* rl = lst + S2S_LINK_BRK_CAP;
+                    for (uint32_t i = lane; i + 1 < r_step; i += 32) {
+                        const uint32_t open = rl[i], next = rl[i + 1];
+                        sm.tstage[open - sslot] = R | (tb + next);
+                        sm.tstage[next - 1 - sslot] = R | (tb + open);
+                    }
+                    const uint32_t a = run.rec + 1, b = run.rec + r_step;  // records [a, b)
+                    const uint32_t wd = (a >> 5) + lane;
+                    if (wd <= ((b - 1) >> 5)) {
+                        const uint32_t lo = wd == (a >> 5) ? (a & 31u) : 0u, hi = wd == ((b - 1) >> 5) ? ((b - 1) & 31u) : 31u;
+                        const uint32_t m = (0xffffffffu >> (31 - hi)) & ~((1u << lo) - 1u);  // bits [lo, hi]
+                        wp.atomic_and(p.rootlink + wd, ~m);
+                    }
+                }
+                wp.sync();
+            }
+            // copy-out: staging word i is tape word sslot + i; the 16-byte aligned middle as vectors (8 lanes fill a
+            // 128-byte line), at most one single word at each end
+            if (w_step) {
+                uint64_t* const d = p.tape + slot0;  // d[i - ph] <-> tstage[i]
+                const uint32_t end = ph + w_step, a = (ph + 1) & ~1u, e = end & ~1u;
+                if (lane == 0 && (ph & 1u)) d[0] = sm.tstage[ph];
+                const V16* s16 = reinterpret_cast<const V16*>(sm.tstage + a);
+                V16* d16 = reinterpret_cast<V16*>(d + (a - ph));
+                for (uint32_t i = lane; i < (e - a) / 2; i += 32) d16[i] = s16[i];
+                if (lane == 31 && (end & 1u)) d[e - ph] = sm.tstage[e];
+            }
+        }
+        wp.sync();  // the staging areas and the escape scratch are reused by the next step
         run.w += w_step;
         run.str += k_step;
         run.brk += b_step;

@@ -5,9 +5,10 @@
 //                      last stage-1 structurals, numbers, bytes behind the last quote)
 //   K2q scan_*_kernel<SlabAgg> (stage2_common.cuh)   exclusive scan of the aggregates (groups of 1024 + their
 //                      totals), grand totals -> Stage2Result
-//   K2r s2s_emit       the same analysis again, now with every offset known: tape words, Strings.B bytes (compacted in
-//                      shared memory and streamed out with coalesced / 16-byte stores), bracket records for the scope
-//                      matching, number list, per-segment grammar masks
+//   K2r s2s_emit       the same analysis again, now with every offset known: tape words and Strings.B bytes (both
+//                      staged in shared memory and streamed out with coalesced / 16-byte stores), the cross-links and
+//                      root words of the pairs inside one step, bracket records for the scope matching, number list,
+//                      per-segment grammar masks
 //   K2h s2s_numbers    parse_number (parse_number.go:65) over the number list, one number per thread
 //   K2d s2_min32 + s2_ansv (stage2_common.cuh)    scope matching on the brackets
 //   K2e s2s_link       per bracket: cross-links of { } [ ] (stage2...go:327-334) and the grammar verdict of the segment
@@ -93,15 +94,17 @@ __global__ void __launch_bounds__(S2_THREADS) s2s_numbers_kernel(const uint8_t* 
 // ones behind bracket k-1 up to and including bracket k -- allowed inside the container that is open there?  That
 // container is the scope open right after bracket k-1: the bracket itself if it opens, else the parent of the scope
 // it closes (par = nearest previous bracket with a smaller depth in front of it, K2d).  Closing brackets cross-link
-// the tape words of their pair (stage2...go:327-334).
+// the tape words of their pair (stage2...go:327-334), except those K2r has linked already (BRK_LINKED: both ends in
+// one staged step).
 // ---------------------------------------------------------------------------------
 // The same launch writes the root words (K2f, stage2...go:170,207-218,428-441): record r opens at rootpos[r], its close
-// sits right in front of the next record's open (or is the last word of the tape).
+// sits right in front of the next record's open (or is the last word of the tape).  Records whose bit in rootlink K2r
+// has cleared are written already.
 __global__ void __launch_bounds__(S2_THREADS) s2s_link_kernel(const S2sParams p, const int32_t* par, uint32_t nb, uint64_t n_records,
                                                               uint64_t tape_len) {
     const uint32_t k = blockIdx.x * S2_THREADS + threadIdx.x;
     const uint64_t tape_base = s2s_tape_base(p);
-    if (k <= n_records) {
+    if (k <= n_records && ((p.rootlink[k >> 5] >> (k & 31)) & 1u)) {
         const uint64_t R = (uint64_t)'r' << 56;
         const uint64_t open = k == 0 ? 0 : p.rootpos[k];
         const uint64_t next_open = k == n_records ? tape_len : p.rootpos[k + 1];
@@ -113,7 +116,7 @@ __global__ void __launch_bounds__(S2_THREADS) s2s_link_kernel(const S2sParams p,
     if (k > nb) return;
     uint32_t ctx = CTX_ROOT;
     if (k > 0) {
-        const uint32_t kd = p.brk_kind[k - 1];
+        const uint32_t kd = p.brk_kind[k - 1] & ~BRK_LINKED;
         int32_t enc;
         if (kd == T_OBJ_OPEN || kd == T_ARR_OPEN) {
             enc = (int32_t)k - 1;
@@ -121,12 +124,12 @@ __global__ void __launch_bounds__(S2_THREADS) s2s_link_kernel(const S2sParams p,
             const int32_t m = par[k - 1];
             enc = m >= 0 ? par[m] : -1;
         }
-        ctx = enc >= 0 ? (p.brk_kind[enc] == T_OBJ_OPEN ? CTX_OBJ : CTX_ARR) : CTX_ROOT;
+        ctx = enc >= 0 ? ((p.brk_kind[enc] & ~BRK_LINKED) == T_OBJ_OPEN ? CTX_OBJ : CTX_ARR) : CTX_ROOT;
     }
     const uint32_t sg = (p.segmask[k >> 2] >> (8 * (k & 3))) & 0xffu;
     if (!((sg >> ctx) & 1u)) atomicOr(p.error, 1u);
     if (k < nb) {
-        const uint32_t kd = p.brk_kind[k];
+        const uint32_t kd = p.brk_kind[k];  // (a linked close carries BRK_LINKED and matches neither kind)
         if (kd == T_OBJ_CLOSE || kd == T_ARR_CLOSE) {
             const int32_t m = par[k];
             if (m >= 0) {
