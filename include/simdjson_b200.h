@@ -189,6 +189,68 @@ int sj_parse_count_where(sj_ctx* ctx, const uint8_t* msg, size_t len, uint32_t f
                          size_t key_len, const uint8_t* value, size_t value_len, uint64_t* roots, uint64_t* matches);
 
 /*
+ * ForEach + FindElement on the device: for every root of a tape (in tape order: one per NDJSON record, one for a single
+ * document) and every path, the value at that path, read into typed columns in device memory.  A cell is a literal
+ * port of ParsedJson.ForEach (parsed_json.go:125-138) handing each root's element to Iter.FindElement(path...)
+ * (:833-864 -> Iter.Object :998-1018 -> Object.FindPath parsed_object.go:256-316), then the accessor of the path's kind:
+ *   SJ_FIND_KIND_ELEMENT  none               SJ_FIND_KIND_INT64   Iter.Int    (:629-661)
+ *   SJ_FIND_KIND_UINT64   Iter.Uint (:679-712) SJ_FIND_KIND_FLOAT64 Iter.Float (:560-583)
+ *   SJ_FIND_KIND_BOOL     Iter.Bool (:867-875) SJ_FIND_KIND_STRING  Iter.StringBytes (:741-749)
+ * So the first member with the key decides, keys compare on their unescaped bytes, arrays are never entered, and a
+ * root or intermediate value that is not an object is SJ_FIND_NOT_OBJECT, not SJ_FIND_NOT_FOUND.  Where amd64 Go and
+ * CUDA's conversions differ the cell follows Go: Int() of a float of exactly 2^63 is math.MinInt64 (CVTTSD2SQ), Uint()
+ * of exactly 2^64 is 1<<63 (Go's float64ToUint64 lowering).
+ * Cell status (u8): SJ_FIND_OK found and converted; SJ_FIND_NOT_FOUND ErrPathNotFound (also a path of 0 segments);
+ * SJ_FIND_NOT_OBJECT "type ... found before object" / "value of key ... is not an object"; SJ_FIND_CONVERT the accessor's
+ * error; SJ_FIND_CORRUPT any other error (or panic) of the reference on a malformed tape.  Tag (u8): the found element's
+ * tag byte; index (i64): the tape index of its head word (-1 and tag 0 when nothing was found); value (8 bytes): int64,
+ * uint64, the bits of a float64, 0 / 1 for BOOL, the byte length for STRING, 0 for ELEMENT and for cells not OK.
+ * Layout, path-major with a row stride of row_cap: cell (p, r) of status / tag / index / value is at p * row_cap + r;
+ * STRING path s (counting STRING paths only, in path order) has str_offsets[s * (row_cap + 1) + r], r = 0 .. rows, into
+ * str_bytes, so row r's bytes are [off[r], off[r + 1]) (with no rows, the one entry 0 is written when str_offsets is given).
+ * Limits: 1 to 64 paths, 0 to 32 segments each, 16 KiB of segment bytes in all; else SJ_ERR_ARGUMENT.  A tape longer
+ * than 2^32 - 1 words returns SJ_ERR_TOO_LARGE.  *rows and *str_bytes are exact even on SJ_ERR_CAPACITY (rows > row_cap
+ * or str_bytes > str_cap), when nothing is written; out may be NULL to ask for the sizes.
+ * sj_find_device: message, tape, strings and out in device memory, with their lengths (every read stays inside them).
+ * On the tape this context's last parse left in HBM the rows are stage 2's root list; on any other tape they are found
+ * on the device: the 'r' words that point forward and are not the value word of a string or number (read from word 0),
+ * which on every tape the parser or sj_deserialize_device writes are the roots ForEach visits.  sj_parse_find: HOST message in, parse and find on the device, only the columns are copied to `out`
+ * (host memory); parse errors return the parse codes.
+ */
+#define SJ_FIND_OK 0
+#define SJ_FIND_NOT_FOUND 1
+#define SJ_FIND_NOT_OBJECT 2
+#define SJ_FIND_CONVERT 3
+#define SJ_FIND_CORRUPT 4
+#define SJ_FIND_KIND_ELEMENT 0
+#define SJ_FIND_KIND_INT64 1
+#define SJ_FIND_KIND_UINT64 2
+#define SJ_FIND_KIND_FLOAT64 3
+#define SJ_FIND_KIND_BOOL 4
+#define SJ_FIND_KIND_STRING 5
+typedef struct {
+    const uint8_t* segments;   /* the key segments laid end to end (host memory) */
+    const uint32_t* seg_lens;  /* n_segments lengths */
+    uint32_t n_segments;
+    uint32_t kind;             /* SJ_FIND_KIND_* */
+} sj_find_path;
+typedef struct {
+    uint8_t* status;       /* [n_paths][row_cap] */
+    uint8_t* tag;          /* [n_paths][row_cap] */
+    int64_t* index;        /* [n_paths][row_cap] */
+    uint64_t* value;       /* [n_paths][row_cap] */
+    int64_t* str_offsets;  /* [STRING paths][row_cap + 1] */
+    uint8_t* str_bytes;    /* str_cap bytes */
+    size_t row_cap;
+    size_t str_cap;
+} sj_find_out;
+int sj_find_device(sj_ctx* ctx, const uint8_t* d_msg, size_t msg_len, const uint64_t* d_tape, size_t tape_len,
+                   const uint8_t* d_strings, size_t strings_len, const sj_find_path* paths, size_t n_paths,
+                   const sj_find_out* out, size_t* rows, size_t* str_bytes);
+int sj_parse_find(sj_ctx* ctx, const uint8_t* msg, size_t len, uint32_t flags, const sj_find_path* paths, size_t n_paths,
+                  const sj_find_out* out, size_t* rows, size_t* str_bytes);
+
+/*
  * MarshalJSON on the device: Iter.MarshalJSON of a fresh pj.Iter() (parsed_json.go:394-556), byte for byte.  Every
  * root's value as compact JSON, roots joined by one '\n' (no trailing newline); strings escaped like escapeBytes, floats
  * like appendFloat (shortest round-trip digits; fixed notation for 1e-6 <= |x| < 1e21 and 0, else d.ddde+-N).

@@ -8,12 +8,17 @@
 // With the tape built in HBM the walk can stay there too: the answer is two integers, so the
 // D2H copy of a tape 1.7x the size of the input (the PCIe leg that bounds sj_parse) disappears.
 //
-//   KC1 tc_find_roots    any device tape: every root-open word ('r' whose payload points forward)
-//                        is appended to a list (warp-aggregated atomics; order is irrelevant for counts)
+//   KC1a tc_root_count   any device tape: root-open words ('r' whose payload points forward, and a head: not
+//                        the value word of a string or number, by KM1 mj_heads_reduce and its scans) per tile
+//                        of MJ_TILE words, whose counts scan_groups_kernel scans (twice).  On every tape the
+//                        parser or Deserialize writes these are the roots ForEach visits.
+//   KC1b tc_root_write   their slots, in tape order (the rows of the device find, find.cuh)
 //   KC2 tc_count_where   one thread per root: FindKey over the top-level keys of the record's
 //                        object, first match decides (FindKey returns the first element of that name)
 #pragma once
 #include "common.cuh"
+#include "marshal.cuh"
+#include "stage2_common.cuh"
 
 namespace sj {
 
@@ -32,27 +37,56 @@ struct CountParams {
     uint32_t key_len;
     const uint8_t* value;
     uint32_t value_len;
-    unsigned long long* counters;  // [0] roots found (KC1), [1] matches
+    unsigned long long* counters;  // [1] matches
 };
 
-__global__ void __launch_bounds__(256) tc_find_roots_kernel(const uint64_t* tape, uint64_t tape_len, uint32_t* roots,
-                                                            uint64_t cap, unsigned long long* counters) {
-    const uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
-    bool is_open = false;
-    if (i < tape_len) {
-        const uint64_t w = tape[i];
-        is_open = (w >> 56) == 'r' && (w & TC_VALUE_MASK) > i;  // the closing root word points backwards
+__device__ __forceinline__ bool tc_is_root_open(uint64_t w, uint64_t i) { return (w >> 56) == 'r' && (w & TC_VALUE_MASK) > i; }
+
+// which of a thread's MJ_ROUNDS consecutive words are root opens: 'r' words pointing forward that are heads, i.e. not the
+// value word of the string or number in front of them (KM1's transfer function, scanned from word 0).  A number whose
+// value word happens to start with the byte 'r' (int64s from 0x72 << 56, doubles near 1e241-1e246) is no root.
+__device__ __forceinline__ uint32_t tc_root_opens(const uint64_t* tape, uint64_t n, const HAgg* h_tile_pre, const HAgg* h_grp_pre,
+                                                  uint64_t base) {
+    uint64_t w[MJ_ROUNDS];
+    HAgg a{};
+#pragma unroll
+    for (int j = 0; j < MJ_ROUNDS; j++) {
+        w[j] = base + j < n ? tape[base + j] : 0;
+        if (base + j < n) a = agg_combine(a, mj_word_agg(w[j], base + j));
     }
-    const uint32_t m = __ballot_sync(FULL, is_open);
-    if (m == 0) return;
-    const uint32_t lane = threadIdx.x & 31;
-    unsigned long long base = 0;
-    if (lane == 0) base = atomicAdd(&counters[0], (unsigned long long)__popc(m));
-    base = __shfl_sync(FULL, base, 0);
-    if (is_open) {
-        const uint64_t slot = base + __popc(m & lanemask_lt());
-        if (slot < cap) roots[slot] = (uint32_t)i;
+    HAgg total;
+    const HAgg ex = block_exclusive_scan(a, total);
+    HAgg pre = agg_combine(agg_combine(h_grp_pre[blockIdx.x >> 10], h_tile_pre[blockIdx.x]), ex);
+    uint32_t open = 0;
+#pragma unroll
+    for (int j = 0; j < MJ_ROUNDS; j++) {
+        if (base + j < n && hagg_out(pre, 1) && tc_is_root_open(w[j], base + j)) open |= 1u << j;
+        pre = agg_combine(pre, mj_word_agg(w[j], base + j));
     }
+    return open;
+}
+
+// KC1a: root opens per tile of MJ_TILE words (MJ_ROUNDS consecutive words per thread), after KM1 and its scans
+__global__ void __launch_bounds__(MJ_THREADS) tc_root_count_kernel(const uint64_t* tape, uint64_t n, const HAgg* h_tile_pre,
+                                                                   const HAgg* h_grp_pre, MSum* tile) {
+    const uint64_t base = (uint64_t)blockIdx.x * MJ_TILE + (uint64_t)threadIdx.x * MJ_ROUNDS;
+    const uint32_t open = tc_root_opens(tape, n, h_tile_pre, h_grp_pre, base);
+    MSum total;
+    block_exclusive_scan(MSum{(uint64_t)__popc(open)}, total);
+    if (threadIdx.x == 0) tile[blockIdx.x] = total;
+}
+
+// KC1b: the slots, in tape order
+__global__ void __launch_bounds__(MJ_THREADS) tc_root_write_kernel(const uint64_t* tape, uint64_t n, const HAgg* h_tile_pre,
+                                                                   const HAgg* h_grp_pre, const MSum* tile_pre,
+                                                                   const MSum* grp_pre, uint32_t* roots) {
+    const uint64_t base = (uint64_t)blockIdx.x * MJ_TILE + (uint64_t)threadIdx.x * MJ_ROUNDS;
+    const uint32_t open = tc_root_opens(tape, n, h_tile_pre, h_grp_pre, base);
+    MSum total;
+    uint64_t at = grp_pre[blockIdx.x >> 10].v + tile_pre[blockIdx.x].v + block_exclusive_scan(MSum{(uint64_t)__popc(open)}, total).v;
+#pragma unroll
+    for (int j = 0; j < MJ_ROUNDS; j++)
+        if (open >> j & 1) roots[at++] = (uint32_t)(base + j);
 }
 
 // the bytes of the string whose first tape word is w (parsed_json.go:107-120 stringByteAt)

@@ -74,8 +74,10 @@ struct sj_ctx {
     int s2_impl = 0;  // stage 2: 0 = streaming kernels (stage2_stream.cuh) when copy_strings is on, 1 = per-structural kernels (stage2.cuh) always
     DevBuf s2a, s2b, s2c;  // s2a/s2b: stage-2 scratch (before / after the totals are known), s2c: backslash block map
     DevBuf tape, strings;  // device outputs for the host-buffer API
-    // tape consumers (consume.cuh): needles + counters, root list of a foreign tape
-    DevBuf tc_small, tc_roots;
+    // tape consumers (consume.cuh, find.cuh): needles + counters, root list of a foreign tape and the scan that orders it
+    DevBuf tc_small, tc_roots, tc_scan;
+    // device find (find.cuh): paths + counters, per-cell scratch, the columns of sj_parse_find before their copy to the host
+    DevBuf fd_small, fd, fd_out;
     // device MarshalJSON (marshal.cuh): scratch of the passes, the text of sj_parse_marshal before its copy to the host
     DevBuf mj, mj_out;
     // device Serializer (serialize.cuh): scratch of the word passes, of the string dedup, the stream of sj_parse_serialize

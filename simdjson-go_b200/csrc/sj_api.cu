@@ -5,11 +5,13 @@
 // sm_90a kernels of stage1.cuh and of the two stage-2 implementations (stage2_stream.cuh,
 // stage2.cuh; what both run is in stage2_common.cuh).  There is NO CPU fallback: without a
 // CUDA device every entry point returns SJ_ERR_NO_DEVICE.
+#include <algorithm>
 #include <chrono>
 #include <cstdio>
 #include <cstdlib>
 #include <cstring>
 #include <new>
+#include <vector>
 
 #include <sched.h>
 #include <sys/syscall.h>
@@ -21,6 +23,7 @@
 #include "stage2_stream.cuh"
 #include "stage2.cuh"
 #include "consume.cuh"
+#include "find.cuh"
 #include "marshal.cuh"
 #include "serialize.cuh"
 #include "gen.cuh"
@@ -208,7 +211,8 @@ extern "C" void sj_ctx_destroy(sj_ctx* c) {
     exchange_release(c);
     DevBuf* bufs[] = {&c->msg,     &c->idx,     &c->desc,    &c->result,   &c->s2a,      &c->s2b,      &c->s2c,
                       &c->tape,    &c->strings, &c->test_in, &c->test_out, &c->test_aux, &c->tc_small, &c->tc_roots,
-                      &c->mj,      &c->mj_out,  &c->sz,      &c->sz_tab,   &c->sz_out};
+                      &c->tc_scan, &c->fd_small, &c->fd,     &c->fd_out,   &c->mj,       &c->mj_out,   &c->sz,
+                      &c->sz_tab,  &c->sz_out};
     for (DevBuf* b : bufs) b->release();
     if (c->host_result) cudaFreeHost(c->host_result);
     free(c->pending);
@@ -537,6 +541,7 @@ extern "C" int sj_test_flatten_bits(sj_ctx* c, const uint64_t* masks, size_t nma
 #include "sj_parse.inl"
 #include "sj_consume.inl"
 #include "sj_marshal.inl"
+#include "sj_find.inl"
 #include "sj_serialize.inl"
 #include "sj_stream.inl"
 #include "sj_gen.inl"

@@ -10,8 +10,9 @@ import ctypes as C
 import numpy as np
 
 from . import _lib
-from ._lib import (ERR_CAPACITY, ERR_STAGE1, ERR_STAGE2, ERR_UNSUPPORTED, FLAG_COPY_STRINGS, FLAG_NDJSON, OK, SjError,
-                   Stage1Info)
+from ._lib import (ERR_CAPACITY, ERR_STAGE1, ERR_STAGE2, ERR_UNSUPPORTED, FIND_CONVERT, FIND_CORRUPT, FIND_KIND_BOOL,
+                   FIND_KIND_ELEMENT, FIND_KIND_FLOAT64, FIND_KIND_INT64, FIND_KIND_STRING, FIND_KIND_UINT64,
+                   FIND_NOT_FOUND, FIND_NOT_OBJECT, FIND_OK, FLAG_COPY_STRINGS, FLAG_NDJSON, OK, SjError, Stage1Info)
 
 JSONVALUEMASK = 0xFF_FFFF_FFFF_FFFF  # parsed_json.go:26
 JSONTAGOFFSET = 56
@@ -108,6 +109,70 @@ class Context:
         if rc != OK:
             raise SjError(rc)
         return rc, roots.value, matches.value
+
+    def parse_find(self, msg, paths, kinds, ndjson=True, copy_strings=True):
+        """parseMessage + ForEach(FindElement(path...) + the accessor of each kind) (ndjson_test.go:294-315) with the tape
+        left in HBM: (rc, rows, columns).  `paths` is a list of key paths (each a list of byte strings), `kinds` the
+        FIND_KIND_* of each.  columns[p] is a FindColumn of numpy arrays (status, tag, index, value, offsets, data):
+        `value` is int64 / uint64 / float64 by kind (int64 for ELEMENT, BOOL and STRING, where it is the length); a
+        STRING column's row r is data[offsets[r]:offsets[r + 1]].  Only the columns are copied back; on a parse error
+        rows is 0 and columns is None."""
+        m = _as_u8(msg)
+        flags = (FLAG_NDJSON if ndjson else 0) | (FLAG_COPY_STRINGS if copy_strings else 0)
+        cpaths, keep = _find_paths(paths, kinds)
+        rows, nbytes = C.c_size_t(0), C.c_size_t(0)
+        # rows: one per record (records are separated by newlines) or the one document; strings: at most the input per
+        # STRING path, guessed at its size -- else once more at the exact sizes
+        row_cap = int(np.count_nonzero(m == 10)) + 1 if ndjson else 1
+        str_cap = m.size + 64
+        n_str = sum(k == FIND_KIND_STRING for k in kinds)
+        for _ in range(2):
+            cols = (np.empty((len(paths), row_cap), np.uint8), np.empty((len(paths), row_cap), np.uint8),
+                    np.empty((len(paths), row_cap), np.int64), np.empty((len(paths), row_cap), np.uint64),
+                    np.empty((n_str, row_cap + 1), np.int64), np.empty(max(str_cap, 1), np.uint8))
+            out = _lib.FindOut(*(_addr(a) for a in cols), row_cap, str_cap)
+            rc = self.L.sj_parse_find(self.h, _addr(m) if m.size else None, m.size, flags, cpaths, len(paths), C.byref(out),
+                                      C.byref(rows), C.byref(nbytes))
+            if rc != ERR_CAPACITY:
+                break
+            row_cap, str_cap = rows.value, nbytes.value
+        if rc in (ERR_STAGE1, ERR_STAGE2):
+            return rc, 0, None
+        if rc != OK:
+            raise SjError(rc)
+        return rc, rows.value, _find_columns(cols, rows.value, kinds, lambda a, dt: a.view(dt))
+
+    def find_device(self, tape, strings, message, paths, kinds, out=None):
+        """ForEach + FindElement + accessors over a tape already on this context's device (torch tensors as for
+        marshal_device).  `out` (optional) is a tuple of tensors (status u8 [P, R], tag u8 [P, R], index i64 [P, R],
+        value i64 [P, R], str_offsets i64 [S, R + 1], str_bytes u8 [B]) for P paths, S of them STRING, R >= rows;
+        without it they are allocated at the exact sizes.  Returns (rc, rows, columns): columns[p] is a FindColumn of
+        tensor views (value viewed as float64 for FLOAT64 and uint64 for UINT64), or None unless rc is OK.  rc is
+        SJ_ERR_CAPACITY when `out` is too small (rows and the byte total are still exact, in `rows` and nothing written)."""
+        import torch
+        cpaths, keep = _find_paths(paths, kinds)
+        sp, sl = _ptr_len(strings)
+        mp, ml = _ptr_len(message)
+        tp, tl = _ptr_len(tape)
+        rows, nbytes = C.c_size_t(0), C.c_size_t(0)
+        n_str = sum(k == FIND_KIND_STRING for k in kinds)
+        if out is None:
+            rc = self.L.sj_find_device(self.h, mp, ml, tp, tl, sp, sl, cpaths, len(paths), None, C.byref(rows), C.byref(nbytes))
+            if rc not in (OK, ERR_CAPACITY):
+                return rc, rows.value, None
+            dev, R = tape.device, rows.value
+            out = (torch.empty((len(paths), R), dtype=torch.uint8, device=dev), torch.empty((len(paths), R), dtype=torch.uint8, device=dev),
+                   torch.empty((len(paths), R), dtype=torch.int64, device=dev), torch.empty((len(paths), R), dtype=torch.int64, device=dev),
+                   torch.empty((n_str, R + 1), dtype=torch.int64, device=dev), torch.empty(max(nbytes.value, 1), dtype=torch.uint8, device=dev))
+        row_cap = out[0].shape[1]
+        for t, shape in zip(out[:5], [(len(paths), row_cap)] * 4 + [(n_str, row_cap + 1)]):
+            if tuple(t.shape) != shape or not t.is_contiguous():
+                raise ValueError("find_device: out tensors must be contiguous with shapes %s" % shape)
+        o = _lib.FindOut(*(t.data_ptr() for t in out), row_cap, out[5].numel())
+        rc = self.L.sj_find_device(self.h, mp, ml, tp, tl, sp, sl, cpaths, len(paths), C.byref(o), C.byref(rows), C.byref(nbytes))
+        if rc != OK:
+            return rc, rows.value, None
+        return rc, rows.value, _find_columns(out, rows.value, kinds, _torch_view)
 
     def parse_marshal(self, msg, ndjson=False, copy_strings=True):
         """parseMessage + Iter.MarshalJSON (parsed_json.go:394) with the tape left in HBM: (rc, JSON text bytes).  Only
@@ -322,6 +387,54 @@ class Context:
 
 def _ptr_len(t):
     return (t.data_ptr(), t.numel()) if t is not None and t.numel() else (None, 0)
+
+
+class FindColumn(tuple):
+    """one path's column: status, tag, index, value per row; offsets / data for STRING (else None)"""
+    __slots__ = ()
+    _fields = ("status", "tag", "index", "value", "offsets", "data")
+
+    def __new__(cls, *a):
+        return tuple.__new__(cls, a)
+
+    status = property(lambda s: s[0])
+    tag = property(lambda s: s[1])
+    index = property(lambda s: s[2])
+    value = property(lambda s: s[3])
+    offsets = property(lambda s: s[4])
+    data = property(lambda s: s[5])
+
+
+def _find_paths(paths, kinds):
+    """the sj_find_path array (and the buffers it points into)"""
+    if len(paths) != len(kinds):
+        raise ValueError("one kind per path")
+    arr = (_lib.FindPath * max(len(paths), 1))()
+    keep = []
+    for i, (path, kind) in enumerate(zip(paths, kinds)):
+        segs = [bytes(s) for s in path]
+        blob = C.create_string_buffer(b"".join(segs) or b"\0")
+        lens = (C.c_uint32 * max(len(segs), 1))(*[len(s) for s in segs])
+        keep += [blob, lens]
+        arr[i] = _lib.FindPath(C.cast(blob, C.c_void_p), lens, len(segs), int(kind))
+    return arr, keep
+
+
+def _torch_view(a, dt):
+    import torch
+    return a.view({np.float64: torch.float64, np.uint64: torch.uint64, np.int64: torch.int64}[dt])
+
+
+def _find_columns(out, rows, kinds, view):
+    status, tag, index, value, offs, data = out
+    cols, s = [], 0
+    for p, k in enumerate(kinds):
+        dt = np.float64 if k == FIND_KIND_FLOAT64 else np.uint64 if k == FIND_KIND_UINT64 else np.int64
+        o = d = None
+        if k == FIND_KIND_STRING:
+            o, d, s = offs[s, :rows + 1], data, s + 1
+        cols.append(FindColumn(status[p, :rows], tag[p, :rows], index[p, :rows], view(value[p, :rows], dt), o, d))
+    return cols
 
 
 _default_ctx = None

@@ -21,11 +21,15 @@ EXPORTS = [
     "sj_host_free", "sj_trim_space", "sj_bounds", "sj_parse", "sj_parse_device", "sj_gen_ndjson_device", "sj_parse_nd_sharded_count", "sj_parse_nd_sharded_emit", "sj_exchange_create", "sj_exchange_set_gap", "sj_exchange_set_timeout_ms", "sj_exchange_connect", "sj_exchange_connect_ptrs", "sj_exchange_local", "sj_exchange_bases", "sj_exchange_result", "sj_find_structural_indices", "sj_stage1_device",
     "sj_stage1_launch", "sj_ctx_sync", "sj_event_record", "sj_event_elapsed_ms", "sj_kernel_launches",
     "sj_test_block_masks", "sj_test_geometry", "sj_test_finalize", "sj_test_flatten_bits", "sj_test_parse_strings",
-    "sj_test_parse_numbers", "sj_count_where_device", "sj_parse_count_where", "sj_marshal_device", "sj_parse_marshal", "sj_serialize_device", "sj_parse_serialize",
+    "sj_test_parse_numbers", "sj_count_where_device", "sj_parse_count_where", "sj_find_device", "sj_parse_find", "sj_marshal_device", "sj_parse_marshal", "sj_serialize_device", "sj_parse_serialize",
     "sj_deserialize_device", "sj_test_set_string_hash_bits", "sj_test_stage2_internal", "sj_stream_create", "sj_stream_destroy",
     "sj_stream_write", "sj_stream_close_input", "sj_stream_next", "sj_stream_release",
 ]
 STREAM_END, STREAM_EMPTY, STREAM_BUSY = 7, 8, 9
+# sj_find_device / sj_parse_find: cell statuses and path kinds
+FIND_OK, FIND_NOT_FOUND, FIND_NOT_OBJECT, FIND_CONVERT, FIND_CORRUPT = range(5)
+FIND_KIND_ELEMENT, FIND_KIND_INT64, FIND_KIND_UINT64, FIND_KIND_FLOAT64, FIND_KIND_BOOL, FIND_KIND_STRING = range(6)
+FIND_MAX_PATHS, FIND_MAX_SEGMENTS, FIND_MAX_SEGMENT_BYTES = 64, 32, 16384
 
 
 class StreamResult(C.Structure):
@@ -35,6 +39,16 @@ class StreamResult(C.Structure):
 
 class ShardTotals(C.Structure):
     _fields_ = [("msg_bytes", C.c_uint64), ("tape_words", C.c_uint64), ("string_bytes", C.c_uint64), ("records", C.c_uint64)]
+
+
+class FindPath(C.Structure):
+    _fields_ = [("segments", C.c_void_p), ("seg_lens", C.POINTER(C.c_uint32)), ("n_segments", C.c_uint32),
+                ("kind", C.c_uint32)]
+
+
+class FindOut(C.Structure):
+    _fields_ = [("status", C.c_void_p), ("tag", C.c_void_p), ("index", C.c_void_p), ("value", C.c_void_p),
+                ("str_offsets", C.c_void_p), ("str_bytes", C.c_void_p), ("row_cap", C.c_size_t), ("str_cap", C.c_size_t)]
 
 
 class Stage1Info(C.Structure):
@@ -133,6 +147,10 @@ def load():
     L.sj_count_where_device.argtypes = [vp, vp, vp, sz, vp, C.c_char_p, sz, C.c_char_p, sz, C.POINTER(u64), C.POINTER(u64)]
     L.sj_parse_count_where.restype = i32
     L.sj_parse_count_where.argtypes = [vp, vp, sz, u32, C.c_char_p, sz, C.c_char_p, sz, C.POINTER(u64), C.POINTER(u64)]
+    L.sj_find_device.restype = i32
+    L.sj_find_device.argtypes = [vp, vp, sz, vp, sz, vp, sz, C.POINTER(FindPath), sz, C.POINTER(FindOut), szp, szp]
+    L.sj_parse_find.restype = i32
+    L.sj_parse_find.argtypes = [vp, vp, sz, u32, C.POINTER(FindPath), sz, C.POINTER(FindOut), szp, szp]
     L.sj_marshal_device.restype = i32
     L.sj_marshal_device.argtypes = [vp, vp, sz, vp, sz, vp, sz, vp, sz, szp]
     L.sj_parse_marshal.restype = i32

@@ -1,0 +1,162 @@
+"""Device find (sj_find_device) on the K0 batch: parking-citations-shaped NDJSON generated on the device (sj_gen_ndjson_device),
+ParseND'd into HBM, then ForEach + FindElement with 1, 4 and 16 paths (every key of the record is a STRING path; the
+16-path set is the first 16 keys).  Prints one JSON line per path count:
+  find_ms            sj_find_device, CUDA events around --calls back-to-back calls after --warmup calls
+  parse_ms           sj_parse_device of the same input, timed the same way
+  launches_per_call  kernels per sj_find_device call (the context's counter)
+  min_bytes          the least the algorithm moves: the tape read once, the string bytes read and written, and the
+                     columns written (18 bytes per cell, 8 per STRING offset); min_gbs = min_bytes / find time
+  host rates         sj_parse_find, sj_parse and sj_parse_count_where host to host, wall clock, GB/s of input
+The card's name and power limit are read in the same run.
+usage: python tools/find_bench.py [--mib 512] [--calls 10] [--warmup 3]"""
+import argparse
+import ctypes as C
+import json
+import os
+import subprocess
+import sys
+import time
+
+ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+sys.path.insert(0, ROOT)
+sys.path.insert(0, os.path.join(ROOT, "simdjson-go_b200"))
+
+
+def card():
+    out = subprocess.run(["nvidia-smi", "-i", "0", "--query-gpu=name,power.limit", "--format=csv,noheader,nounits"],
+                         capture_output=True, text=True, check=True).stdout.strip()
+    name, limit = [x.strip() for x in out.split(",")]
+    return name, float(limit)
+
+
+def main():
+    ap = argparse.ArgumentParser()
+    ap.add_argument("--mib", type=int, default=512)
+    ap.add_argument("--calls", type=int, default=10)
+    ap.add_argument("--warmup", type=int, default=3)
+    args = ap.parse_args()
+
+    import numpy as np
+    import torch
+    import simdjson_b200 as sj
+    from simdjson_b200 import _find_paths, _lib
+    from tests.util import load_fixture
+
+    assert sj.SupportedCPU(), "no sm_90 device: this benchmark measures the GPU only"
+    name, plimit = card()
+    dev = torch.device("cuda", 0)
+    ctx = sj.Context(0)
+    L = ctx.L
+    ms = C.c_float(0)
+
+    def timed(fn, calls):
+        L.sj_ctx_sync(ctx.h)
+        L.sj_event_record(ctx.h, 0)
+        for _ in range(calls):
+            fn()
+        L.sj_event_record(ctx.h, 1)
+        L.sj_event_elapsed_ms(ctx.h, C.byref(ms))
+        return ms.value / 1e3 / calls
+
+    pk = load_fixture("parking-citations").strip()
+    lines = pk.split(b"\n")
+    keys = [k.encode() for k in json.loads(lines[0])]
+    n_rec = (args.mib << 20) // (len(pk) // len(lines) + 1)
+    d_msg = torch.full(((args.mib << 20) + (4 << 20),), 0x20, dtype=torch.uint8, device=dev)
+    glen = C.c_size_t(0)
+    assert L.sj_gen_ndjson_device(ctx.h, pk, len(pk), 0, n_rec, d_msg.data_ptr(), d_msg.numel() - (1 << 16), C.byref(glen)) == 0
+    n = glen.value
+    flags = _lib.FLAG_NDJSON | _lib.FLAG_COPY_STRINGS
+    tcap, scap = C.c_size_t(0), C.c_size_t(0)
+    L.sj_bounds(n, C.byref(tcap), C.byref(scap))
+    tl, sl = C.c_size_t(0), C.c_size_t(0)
+    d_tape = torch.empty(tcap.value, dtype=torch.int64, device=dev)
+    d_str = torch.empty(scap.value, dtype=torch.uint8, device=dev)
+
+    def parse():
+        r = L.sj_parse_device(ctx.h, d_msg.data_ptr(), n, flags, d_tape.data_ptr(), d_tape.numel(), C.byref(tl),
+                              d_str.data_ptr(), d_str.numel(), C.byref(sl))
+        assert r == 0, r
+
+    for _ in range(args.warmup):
+        parse()
+    t_parse = timed(parse, args.calls)
+    tape_words, strings_len = tl.value, sl.value
+    host_msg = d_msg[:n].cpu().numpy().tobytes()
+    h_in = torch.frombuffer(bytearray(host_msg), dtype=torch.uint8).pin_memory()
+
+    for k in (1, 4, 16):
+        paths, kinds = [[key] for key in keys[:k]], [_lib.FIND_KIND_STRING] * k
+        cp, keep = _find_paths(paths, kinds)
+        rows, nbytes = C.c_size_t(0), C.c_size_t(0)
+        rcap = n_rec + 1
+        out_t = (torch.empty((k, rcap), dtype=torch.uint8, device=dev), torch.empty((k, rcap), dtype=torch.uint8, device=dev),
+                 torch.empty((k, rcap), dtype=torch.int64, device=dev), torch.empty((k, rcap), dtype=torch.int64, device=dev),
+                 torch.empty((k, rcap + 1), dtype=torch.int64, device=dev), torch.empty(n, dtype=torch.uint8, device=dev))
+        out = _lib.FindOut(*(t.data_ptr() for t in out_t), rcap, n)
+
+        def find():
+            # the tape the context just built: rows come from stage 2's root list
+            r = L.sj_find_device(ctx.h, d_msg.data_ptr(), n, d_tape.data_ptr(), tape_words, d_str.data_ptr(), strings_len,
+                                 cp, k, C.byref(out), C.byref(rows), C.byref(nbytes))
+            assert r == 0 and rows.value == n_rec, (r, rows.value)
+
+        parse()  # the host calls of the previous path count parsed into the context's own buffers
+        for _ in range(args.warmup):
+            find()
+        assert bool((out_t[0][:, :n_rec] == 0).all()), "a cell is not OK"
+        l0 = ctx.launches()
+        t_find = timed(find, args.calls)
+        launches = (ctx.launches() - l0) / args.calls
+        cells = k * n_rec
+        min_bytes = tape_words * 8 + 2 * nbytes.value + 18 * cells + 8 * (cells + k)
+
+        # host to host
+        h_cols = (np.empty((k, rcap), np.uint8), np.empty((k, rcap), np.uint8), np.empty((k, rcap), np.int64),
+                  np.empty((k, rcap), np.uint64), np.empty((k, rcap + 1), np.int64), np.empty(n, np.uint8))
+        for a in h_cols:
+            a.fill(0)
+        h_out = _lib.FindOut(*(a.ctypes.data for a in h_cols), rcap, n)
+        h_tape = torch.empty(tape_words + 64, dtype=torch.int64).pin_memory()
+        h_str = torch.empty(strings_len + 64, dtype=torch.uint8).pin_memory()
+        mo_, ml_ = C.c_size_t(0), C.c_size_t(0)
+        roots, matches = C.c_uint64(0), C.c_uint64(0)
+
+        def host_find():
+            r = L.sj_parse_find(ctx.h, h_in.data_ptr(), n, flags, cp, k, C.byref(h_out), C.byref(rows), C.byref(nbytes))
+            assert r == 0, r
+
+        def host_parse():
+            r = L.sj_parse(ctx.h, h_in.data_ptr(), n, flags, h_tape.data_ptr(), h_tape.numel(), C.byref(tl), h_str.data_ptr(),
+                           h_str.numel(), C.byref(sl), C.byref(mo_), C.byref(ml_))
+            assert r == 0, r
+
+        def host_count():
+            r = L.sj_parse_count_where(ctx.h, h_in.data_ptr(), n, flags, b"Make", 4, b"HOND", 4, C.byref(roots), C.byref(matches))
+            assert r == 0, r
+
+        rates = {}
+        for key, fn in (("parse_find", host_find), ("parse", host_parse), ("parse_count_where", host_count)):
+            fn()
+            t0 = time.perf_counter()
+            for _ in range(args.calls):
+                fn()
+            rates[key] = n / ((time.perf_counter() - t0) / args.calls) / 1e9
+
+        print(json.dumps({
+            "input": "K0 gen_ndjson: %d parking-citations-shaped records, ParseND, copy_strings" % n_rec, "input_bytes": n,
+            "tape_words": tape_words, "paths": k, "kind": "STRING", "rows": n_rec, "string_bytes_out": nbytes.value,
+            "find_ms": round(t_find * 1e3, 3), "parse_ms": round(t_parse * 1e3, 3),
+            "launches_per_call": launches, "min_bytes": int(min_bytes), "min_gbs": round(min_bytes / t_find / 1e9, 1),
+            "parse_find_host_gbs": round(rates["parse_find"], 3), "parse_host_e2e_gbs": round(rates["parse"], 3),
+            "parse_count_where_host_gbs": round(rates["parse_count_where"], 3),
+            "timer": "CUDA events around %d back-to-back calls after %d warm-up calls; host rates: wall clock, one context"
+                     % (args.calls, args.warmup),
+            "card": name, "power_limit_w": plimit}), flush=True)
+        del out_t, h_cols, h_tape, h_str
+        torch.cuda.empty_cache()
+    ctx.close()
+
+
+if __name__ == "__main__":
+    main()
