@@ -19,6 +19,9 @@
 
 namespace sj {
 
+// the tape word of a string in Strings.B has it set (not one in the message): stage 2 writes it, tape.cuh reads it
+constexpr uint64_t STRINGBUFBIT = 0x80000000000000ull;  // parsed_json.go:29
+
 // ---------------------------------------------------------------------------------
 // portable "intrinsics"
 // ---------------------------------------------------------------------------------

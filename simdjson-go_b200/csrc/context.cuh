@@ -16,11 +16,11 @@ struct ResultBlock {
     uint8_t gap1[64 - sizeof(sj::Stage1Result)];
     sj::Stage2Result s2;
     uint8_t gap2[128 - sizeof(sj::Stage2Result)];
-    uint64_t counters[2];  // mirror only: where the tape consumers (sj_consume.inl) land their two device counters
+    alignas(16) uint8_t back[128];  // mirror only: where the tape consumers' read-backs land (fetch, sj_tape.inl)
 };
 static_assert(offsetof(ResultBlock, s1) == 0, "result block layout");
 static_assert(offsetof(ResultBlock, s2) == 64, "result block layout");
-static_assert(offsetof(ResultBlock, counters) == 192, "result block layout");
+static_assert(offsetof(ResultBlock, back) == 192, "result block layout");
 
 struct S2Pending;  // sj_parse.inl
 
@@ -74,14 +74,10 @@ struct sj_ctx {
     int s2_impl = 0;  // stage 2: 0 = streaming kernels (stage2_stream.cuh) when copy_strings is on, 1 = per-structural kernels (stage2.cuh) always
     DevBuf s2a, s2b, s2c;  // s2a/s2b: stage-2 scratch (before / after the totals are known), s2c: backslash block map
     DevBuf tape, strings;  // device outputs for the host-buffer API
-    // tape consumers (consume.cuh, find.cuh): needles + counters, root list of a foreign tape and the scan that orders it
-    DevBuf tc_small, tc_roots, tc_scan;
-    // device find (find.cuh): paths + counters, per-cell scratch, the columns of sj_parse_find before their copy to the host
-    DevBuf fd_small, fd, fd_out;
-    // device MarshalJSON (marshal.cuh): scratch of the passes, the text of sj_parse_marshal before its copy to the host
-    DevBuf mj, mj_out;
-    // device Serializer (serialize.cuh): scratch of the word passes, of the string dedup, the stream of sj_parse_serialize
-    DevBuf sz, sz_tab, sz_out;
+    // tape consumers (tape.cuh and its users), each alive within one call only: the call's arguments (countWhere's
+    // needles, the find's paths), the scratch of its passes, the Serializer's string dedup, the root list of a foreign
+    // tape and the scan that finds it, and the output of an sj_parse_* call before its copy to the host
+    DevBuf args, scratch, sz_tab, tc_roots, tc_scan, staging;
     uint32_t sz_hash_bits = 0;  // test hook: keep only this many bits of the dedup hash (0 = all)
     // what the last successful stage 2 of this context left in device memory (valid until the next call)
     const uint32_t* last_rootpos = nullptr;  // stage 2's root list (slot of every record's root-open word, [0] implicit)

@@ -12,7 +12,7 @@
 // of AdvanceInto / AdvanceIter skips at least one word, Advance's at least its own), so a malformed tape terminates.
 //
 // Rows are the roots in tape order: stage 2's root list for the tape the context just built, else KC1a / KC1b
-// (consume.cuh), as for countWhere.
+// (tape.cuh), as for countWhere.
 //   KF3 fd_walk         one thread per (path, row), path-major, the path's segments staged in shared memory; the cell's
 //       status, tag, head index and converted value into scratch, a STRING cell's length into `slen`
 //   KF4 fd_len_reduce   per-tile sums of `slen` (scan_groups_kernel twice)
@@ -20,16 +20,12 @@
 //       longer than FD_SHORT by their whole warp), and the fixed-size columns with the caller's row stride
 #pragma once
 #include "common.cuh"
-#include "marshal.cuh"
-#include "stage2_common.cuh"
+#include "tape.cuh"
 
 namespace sj {
 
 constexpr int FD_THREADS = 256;     // KF3
 constexpr uint64_t FD_SHORT = 32;   // longer strings are copied by their whole warp
-constexpr uint64_t FD_VALUE_MASK = 0x00ffffffffffffffull;   // JSONVALUEMASK, parsed_json.go:26
-constexpr uint64_t FD_STRINGBUFBIT = 0x80000000000000ull;   // parsed_json.go:29
-constexpr uint64_t FD_STRINGBUFMASK = 0x7fffffffffffffull;  // parsed_json.go:30
 
 // cell status (SJ_FIND_*) and path kind (SJ_FIND_KIND_*)
 enum : uint32_t { FD_OK = 0, FD_NOT_FOUND = 1, FD_NOT_OBJECT = 2, FD_CONVERT = 3, FD_CORRUPT = 4 };
@@ -45,16 +41,9 @@ struct FdSeg {
 };
 
 struct FindParams {
-    const uint64_t* tape;
-    uint64_t n;
-    const uint8_t* msg;
-    uint64_t msg_len;
-    const uint8_t* strings;
-    uint64_t strings_len;
-    const uint32_t* roots;   // slot of every root-open word, in tape order
-    uint32_t roots_skip0;    // 1: roots[0] is not stored and means slot 0 (stage 2's rootpos array)
+    TapeView t;
+    TapeRows roots;          // one row per root
     uint32_t n_paths;
-    uint64_t rows;
     const FdPath* paths;
     const FdSeg* segs;
     const uint8_t* seg_bytes;
@@ -74,7 +63,6 @@ struct FdIt {
     uint32_t t;
 };
 
-__device__ __forceinline__ bool fd_value_tag(uint32_t t) { return t == '"' || t == 'l' || t == 'u' || t == 'd'; }
 __device__ __forceinline__ bool fd_scope_tag(uint32_t t) { return t == 'r' || t == '{' || t == '['; }
 // TagToType (parsed_json.go:1152-1163): TypeNone = 0; only String (2) and Object (7) are told apart by the walk
 __device__ __forceinline__ uint32_t fd_type(uint32_t t) {
@@ -95,7 +83,7 @@ __device__ __forceinline__ uint32_t fd_type(uint32_t t) {
 // calcNext, parsed_json.go:268-278
 __device__ __forceinline__ void fd_calc_next(FdIt& it, bool into) {
     it.add = 0;
-    if (fd_value_tag(it.t))
+    if (tape_value_tag(it.t))
         it.add = 1;
     else if (!into && fd_scope_tag(it.t))
         it.add = (int64_t)it.cur - (int64_t)it.off;
@@ -115,10 +103,10 @@ __device__ uint32_t fd_advance(const FindParams& p, FdIt& it) {
             it.t = 0;
             return 0;
         }
-        const uint64_t v = p.tape[it.off];
+        const uint64_t v = p.t.tape[it.off];
         it.t = (uint32_t)(v >> 56);
         it.off++;
-        it.cur = v & FD_VALUE_MASK;
+        it.cur = v & TAPE_VALUE_MASK;
         if (it.t == 'N') {
             it.off += it.cur;
             continue;
@@ -142,9 +130,9 @@ __device__ uint32_t fd_advance_into(const FindParams& p, FdIt& it) {
             it.t = 0;
             return 0;
         }
-        const uint64_t v = p.tape[it.off];
+        const uint64_t v = p.t.tape[it.off];
         it.t = (uint32_t)(v >> 56);
-        it.cur = v & FD_VALUE_MASK;
+        it.cur = v & TAPE_VALUE_MASK;
         if (it.t == 'N') {
             if (it.cur == 0) {
                 fd_move_to_end(it);
@@ -171,8 +159,8 @@ __device__ uint32_t fd_advance_iter(const FindParams& p, FdIt& it, FdIt& dst, ui
             return FD_NOT_FOUND;
         }
         if (it.off > it.n) return FD_CORRUPT;  // "offset bigger than tape"
-        const uint64_t v = p.tape[it.off];
-        it.cur = v & FD_VALUE_MASK;
+        const uint64_t v = p.t.tape[it.off];
+        it.cur = v & TAPE_VALUE_MASK;
         it.t = (uint32_t)(v >> 56);
         it.off++;
         if (it.t == 'N') {
@@ -196,19 +184,6 @@ __device__ uint32_t fd_advance_iter(const FindParams& p, FdIt& it, FdIt& dst, ui
     return FD_OK;
 }
 
-// stringByteAt, parsed_json.go:107-120 (an offset + length that wraps makes the reference's slice panic)
-__device__ __forceinline__ bool fd_string(const FindParams& p, uint64_t offset, uint64_t length, const uint8_t** s) {
-    if (!(offset & FD_STRINGBUFBIT)) {
-        if (offset + length < offset || offset + length > p.msg_len) return false;
-        *s = p.msg + offset;
-        return true;
-    }
-    offset &= FD_STRINGBUFMASK;
-    if (offset + length < offset || offset + length > p.strings_len) return false;
-    *s = p.strings + offset;
-    return true;
-}
-
 // Object.FindPath, parsed_object.go:256-316, over the object Tape[:n] whose members start at off; path = nseg >= 1
 // staged segments.  FD_OK: e is the element's Iter, or *fresh when AdvanceIter met the end exactly.
 __device__ uint32_t fd_find_path(const FindParams& p, uint64_t n, uint64_t off, const FdSeg* seg, const uint8_t* bytes,
@@ -218,14 +193,14 @@ __device__ uint32_t fd_find_path(const FindParams& p, uint64_t n, uint64_t off, 
     for (;;) {
         const uint32_t typ = fd_advance(p, tmp);
         if (typ != 2 || tmp.off + 1 >= tmp.n) return FD_NOT_FOUND;
-        const uint64_t offset = tmp.cur, length = p.tape[tmp.off];
+        const uint64_t offset = tmp.cur, length = p.t.tape[tmp.off];
         const uint32_t klen = seg[k].len;
         if (length != klen) {
             if (fd_advance(p, tmp) == 0) return FD_NOT_FOUND;
             continue;
         }
         const uint8_t* name;
-        if (!fd_string(p, offset, length, &name)) return FD_CORRUPT;
+        if (!tape_string(p.t, offset, length, &name)) return FD_CORRUPT;
         const uint8_t* key = bytes + seg[k].off;
         bool eq = true;
         for (uint32_t j = 0; j < klen; j++)
@@ -254,7 +229,7 @@ __device__ uint32_t fd_find_path(const FindParams& p, uint64_t n, uint64_t off, 
 // and Root (:804-824)
 __device__ uint32_t fd_find(const FindParams& p, uint64_t root, const FdSeg* seg, const uint8_t* bytes, uint32_t nseg,
                             FdIt& e, bool* fresh) {
-    FdIt it{p.n, root, 0, 0, 0}, cp{0, 0, 0, 0, 0};
+    FdIt it{p.t.n, root, 0, 0, 0}, cp{0, 0, 0, 0, 0};
     uint32_t typ;
     if (fd_advance_iter(p, it, cp, &typ) != FD_OK) return FD_CORRUPT;  // (the root word is read: never "ended")
     fd_advance_into(p, cp);
@@ -300,14 +275,14 @@ __device__ uint32_t fd_convert(const FindParams& p, const FdIt& e, uint32_t kind
     if (kind == FD_STRING) {  // StringBytes, parsed_json.go:741-749
         if (t != '"') return FD_CONVERT;
         if (e.off >= e.n) return FD_CORRUPT;
-        const uint64_t len = p.tape[e.off];
-        if (!fd_string(p, e.cur, len, s)) return FD_CORRUPT;
+        const uint64_t len = p.t.tape[e.off];
+        if (!tape_string(p.t, e.cur, len, s)) return FD_CORRUPT;
         *val = len;
         return FD_OK;
     }
     if (t != 'd' && t != 'l' && t != 'u') return FD_CONVERT;  // "unable to convert type %v to ..."
     if (e.off >= e.n) return FD_CORRUPT;  // "corrupt input: expected ..., but no more values on tape"
-    const uint64_t pl = p.tape[e.off];
+    const uint64_t pl = p.t.tape[e.off];
     const double d = __longlong_as_double((long long)pl);
     if (kind == FD_FLOAT64) {  // Float, parsed_json.go:560-583
         *val = t == 'd' ? pl : (uint64_t)__double_as_longlong(t == 'l' ? __ll2double_rn((long long)pl) : __ull2double_rn(pl));
@@ -343,11 +318,11 @@ __device__ uint32_t fd_convert(const FindParams& p, const FdIt& e, uint32_t kind
 // the segments of the paths its cells belong to: their descriptors, then their bytes.
 __global__ void __launch_bounds__(FD_THREADS) fd_walk_kernel(const FindParams p) {
     extern __shared__ uint8_t fd_smem[];
-    const uint64_t cells = p.rows * p.n_paths;
+    const uint64_t cells = p.roots.n * p.n_paths;
     const uint64_t q0 = (uint64_t)blockIdx.x * FD_THREADS;
-    const uint32_t p0 = (uint32_t)(q0 / p.rows);
+    const uint32_t p0 = (uint32_t)(q0 / p.roots.n);
     const uint64_t qlast = min(q0 + FD_THREADS, cells) - 1;
-    const uint32_t p1 = (uint32_t)(qlast / p.rows);
+    const uint32_t p1 = (uint32_t)(qlast / p.roots.n);
     const uint32_t s_lo = p.paths[p0].seg0, s_hi = p.paths[p1].seg0 + p.paths[p1].nseg;
     const uint32_t b_lo = s_lo < s_hi ? p.segs[s_lo].off : 0;
     const uint32_t b_hi = s_lo < s_hi ? p.segs[s_hi - 1].off + p.segs[s_hi - 1].len : 0;
@@ -359,10 +334,10 @@ __global__ void __launch_bounds__(FD_THREADS) fd_walk_kernel(const FindParams p)
     __syncthreads();
     const uint64_t q = q0 + threadIdx.x;
     if (q >= cells) return;
-    const uint32_t pi = (uint32_t)(q / p.rows);
-    const uint64_t r = q - (uint64_t)pi * p.rows;
+    const uint32_t pi = (uint32_t)(q / p.roots.n);
+    const uint64_t r = q - (uint64_t)pi * p.roots.n;
     const FdPath path = p.paths[pi];
-    const uint64_t root = (p.roots_skip0 && r == 0) ? 0 : p.roots[r];
+    const uint64_t root = tape_root(p.roots, r);
     FdIt e{0, 0, 0, 0, 0};
     bool fresh = false;
     uint32_t st = fd_find(p, root, sseg + (path.seg0 - s_lo), sbytes, path.nseg, e, &fresh);
@@ -382,25 +357,23 @@ __global__ void __launch_bounds__(FD_THREADS) fd_walk_kernel(const FindParams p)
     p.tag[q] = (uint8_t)tag;
     p.idx[q] = idx;
     p.val[q] = val;
-    if (path.kind == FD_STRING) p.slen[(uint64_t)path.sidx * p.rows + r] = val;
+    if (path.kind == FD_STRING) p.slen[(uint64_t)path.sidx * p.roots.n + r] = val;
 }
 
 // KF4: per-tile sums of slen
-__global__ void __launch_bounds__(MJ_THREADS) fd_len_reduce_kernel(const uint64_t* slen, uint64_t n, MSum* tile) {
-    const uint64_t base = (uint64_t)blockIdx.x * MJ_TILE + (uint64_t)threadIdx.x;
+__global__ void __launch_bounds__(TAPE_THREADS) fd_len_reduce_kernel(const uint64_t* slen, uint64_t n, MSum* tile) {
+    const uint64_t base = (uint64_t)blockIdx.x * TAPE_TILE + (uint64_t)threadIdx.x;
     uint64_t k = 0;
 #pragma unroll
-    for (int j = 0; j < MJ_ROUNDS; j++)
-        if (base + (uint64_t)j * MJ_THREADS < n) k += slen[base + (uint64_t)j * MJ_THREADS];
+    for (int j = 0; j < TAPE_ROUNDS; j++)
+        if (base + (uint64_t)j * TAPE_THREADS < n) k += slen[base + (uint64_t)j * TAPE_THREADS];
     MSum total;
     block_exclusive_scan(MSum{k}, total);
     if (threadIdx.x == 0) tile[blockIdx.x] = total;
 }
 
 struct FindEmit {
-    const uint64_t* tape;
-    const uint8_t* msg;
-    const uint8_t* strings;
+    TapeView t;
     uint64_t rows, row_cap;
     uint32_t n_paths, n_str;
     uint32_t str_ntiles;
@@ -421,14 +394,14 @@ struct FindEmit {
     uint8_t* o_bytes;
 };
 
-// KF5: blocks [0, str_ntiles) write the string offsets and bytes of MJ_TILE string cells each; the blocks behind
-// them copy MJ_TILE cells each of the fixed-size columns to the caller's row stride
-__global__ void __launch_bounds__(MJ_THREADS) fd_emit_kernel(const FindEmit p) {
+// KF5: blocks [0, str_ntiles) write the string offsets and bytes of TAPE_TILE string cells each; the blocks behind
+// them copy TAPE_TILE cells each of the fixed-size columns to the caller's row stride
+__global__ void __launch_bounds__(TAPE_THREADS) fd_emit_kernel(const FindEmit p) {
     const uint32_t lane = threadIdx.x & 31;
     if (blockIdx.x >= p.str_ntiles) {
         const uint64_t cells = p.rows * p.n_paths;
-        for (int j = 0; j < MJ_ROUNDS; j++) {
-            const uint64_t q = (uint64_t)(blockIdx.x - p.str_ntiles) * MJ_TILE + (uint64_t)j * MJ_THREADS + threadIdx.x;
+        for (int j = 0; j < TAPE_ROUNDS; j++) {
+            const uint64_t q = (uint64_t)(blockIdx.x - p.str_ntiles) * TAPE_TILE + (uint64_t)j * TAPE_THREADS + threadIdx.x;
             if (q >= cells) break;
             const uint64_t pi = q / p.rows, r = q - pi * p.rows, o = pi * p.row_cap + r;
             p.o_st[o] = p.st[q];
@@ -439,9 +412,9 @@ __global__ void __launch_bounds__(MJ_THREADS) fd_emit_kernel(const FindEmit p) {
         return;
     }
     const uint64_t n = p.rows * p.n_str;
-    uint64_t carry = p.slen_grp_pre[blockIdx.x >> 10].v + p.slen_tile_pre[blockIdx.x].v;
-    for (int j = 0; j < MJ_ROUNDS; j++) {
-        const uint64_t k = (uint64_t)blockIdx.x * MJ_TILE + (uint64_t)j * MJ_THREADS + threadIdx.x;
+    uint64_t carry = tile_prefix(p.slen_tile_pre, p.slen_grp_pre, blockIdx.x).v;
+    for (int j = 0; j < TAPE_ROUNDS; j++) {
+        const uint64_t k = (uint64_t)blockIdx.x * TAPE_TILE + (uint64_t)j * TAPE_THREADS + threadIdx.x;
         const uint64_t len = k < n ? p.slen[k] : 0;
         MSum total;
         const uint64_t off = carry + block_exclusive_scan(MSum{len}, total).v;
@@ -452,10 +425,8 @@ __global__ void __launch_bounds__(MJ_THREADS) fd_emit_kernel(const FindEmit p) {
             int64_t* col = p.o_off + si * (p.row_cap + 1);
             col[r] = (int64_t)off;
             if (r + 1 == p.rows) col[p.rows] = (int64_t)(off + len);
-            if (len) {  // an OK cell: its head word is a string whose range was checked by KF3
-                const uint64_t w = p.tape[p.idx[(uint64_t)p.str_path[si] * p.rows + r]] & FD_VALUE_MASK;
-                s = (w & FD_STRINGBUFBIT) ? p.strings + (w & FD_STRINGBUFMASK) : p.msg + w;
-            }
+            if (len)  // an OK cell: its head word is a string whose range was checked by KF3
+                s = tape_string_ptr(p.t, p.t.tape[p.idx[(uint64_t)p.str_path[si] * p.rows + r]]);
         }
         uint8_t* d = p.o_bytes + off;
         if (len <= FD_SHORT)

@@ -111,8 +111,6 @@ SJ_HDC uint32_t char_type(uint32_t ch) {
                         : (uint32_t)T_INVALID;
 }
 
-constexpr uint64_t STRINGBUFBIT = 0x80000000000000ull;  // parsed_json.go:29
-
 // 16 bytes moved as one vector access (LDS.128 / LDG.128 / STG.128 on the device)
 struct alignas(16) V16 {
     uint32_t x, y, z, w;

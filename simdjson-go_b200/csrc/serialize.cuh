@@ -17,8 +17,8 @@
 // not depend on thread scheduling nor on where a string's bytes lived (Strings.B or the message), and the message block
 // is never larger than the reference's.
 //
-// Serialize, word-parallel passes over tiles of SZ_TILE words (= marshal.cuh's, so KM1's tile transfer functions serve):
-//   KM1 mj_heads_reduce + scans          which words are heads
+// Serialize, word-parallel passes over tiles of SZ_TILE words (= tape.cuh's, so KM1's tile transfer functions serve):
+//   KM1 mj_heads_reduce + scans (tape.cuh)   which words are heads
 //   KS1 sz_count      checks + per-tile (tag bytes, value bytes, strings)
 //   KS2 sz_index      the tape index of every string, by ordinal
 //   KS3 sz_insert / KS4 sz_resolve, ordinal-parallel, one round per hash salt: every unresolved string's hash class
@@ -31,17 +31,17 @@
 // Deserialize: KD0 dz_header (one thread) reads the block sizes; KD1 dz_count per tag (tape words, value bytes), scanned;
 // KD2 dz_place marks which tag starts at each tape word; KD3 dz_check checks every open's close; KD4 dz_emit writes the tape.
 #pragma once
-#include "marshal.cuh"
+#include "tape.cuh"
 
 namespace sj {
 
-constexpr uint64_t SZ_TILE = 4096;   // words per tile of KS1 / KS2 / KS7 (MJ_TILE: KM1's tile sums are reused)
+constexpr uint64_t SZ_TILE = 4096;   // words per tile of KS1 / KS2 / KS7 (TAPE_TILE: KM1's tile sums are reused)
 constexpr uint64_t SZ_OTILE = 4096;  // strings per tile of KS5 / KS6: 1024 threads x 4
 constexpr int SZ_OTHREADS = 256;     // KS3 / KS4 blocks
 constexpr uint64_t DZ_TILE = 4096;   // tags per tile of KD1 .. KD4: 1024 threads x 4
 constexpr uint32_t SZ_UNRESOLVED = 0xffffffffu;
 constexpr uint64_t SZ_EMPTY = ~0ull;
-static_assert(SZ_TILE == MJ_TILE, "the serialize passes reuse KM1's tiles");
+static_assert(SZ_TILE == TAPE_TILE, "the serialize passes reuse KM1's tiles");
 
 // ---------------------------------------------------------------------------------
 // Serialize
@@ -55,12 +55,7 @@ __device__ __forceinline__ SzSum agg_shfl_up(const SzSum& a, int d) {
 }
 
 struct SerializeParams {
-    const uint64_t* tape;
-    uint64_t n;
-    const uint8_t* msg;
-    uint64_t msg_len;
-    const uint8_t* strings;
-    uint64_t strings_len;
+    TapeView t;
     const HAgg* h_tile_pre;  // KM1's scans
     const HAgg* h_grp_pre;
     SzSum* c_tile;           // KS1 per-tile counts and their scans
@@ -88,56 +83,42 @@ struct SerializeParams {
 // what head word i writes: tag byte, value bytes, 1 if it is a string; false: the reference panics on it
 __device__ __forceinline__ bool sz_item(const SerializeParams& p, uint64_t i, uint64_t w, uint32_t& tag, uint32_t& vals, uint32_t& str) {
     const uint32_t t = (uint32_t)(w >> 56);
-    const uint64_t v = w & MJ_VALUE_MASK;
+    const uint64_t v = w & TAPE_VALUE_MASK;
     tag = t;
     vals = 0;
     str = 0;
     switch (t) {
     case '"': {
-        if (i + 1 >= p.n) return false;
-        const uint64_t len = p.tape[i + 1];
-        const bool sb = (v & MJ_STRINGBUFBIT) != 0;
-        const uint64_t cap = sb ? p.strings_len : p.msg_len, off = v & (MJ_STRINGBUFBIT - 1);
-        if (off > cap || len > cap - off) return false;
+        if (i + 1 >= p.t.n) return false;
+        const uint8_t* s;
+        if (!tape_string(p.t, w, p.t.tape[i + 1], &s)) return false;
         vals = 16;
         str = 1;
         return true;
     }
-    case 'l': case 'u': vals = 8; return i + 1 < p.n;
+    case 'l': case 'u': vals = 8; return i + 1 < p.t.n;
     case 'd':
         if (v) tag = 'e';
         vals = v ? 16 : 8;
-        return i + 1 < p.n;
+        return i + 1 < p.t.n;
     case '{': case '[': case 'r': vals = 8; return true;
     case '}': case ']': case 'n': case 't': case 'f': case 'N': case 0: return true;
     default: return false;
     }
 }
 
-// the words of thread `threadIdx.x` of tile blockIdx.x (SZ_ROUNDS consecutive ones) and the head state in front of them
-constexpr int SZ_ROUNDS = MJ_ROUNDS;
-__device__ __forceinline__ HAgg sz_load(const SerializeParams& p, uint64_t base, uint64_t (&w)[SZ_ROUNDS]) {
-    HAgg a{};
-#pragma unroll
-    for (int j = 0; j < SZ_ROUNDS; j++) {
-        w[j] = base + j < p.n ? p.tape[base + j] : 0;
-        if (base + j < p.n) a = agg_combine(a, mj_word_agg(w[j], base + j));
-    }
-    HAgg total;
-    const HAgg ex = block_exclusive_scan(a, total);
-    return agg_combine(agg_combine(p.h_grp_pre[blockIdx.x >> 10], p.h_tile_pre[blockIdx.x]), ex);
-}
+constexpr int SZ_ROUNDS = TAPE_ROUNDS;  // consecutive words per thread (tape_heads)
 
 // KS1: checks and per-tile counts
-__global__ void __launch_bounds__(MJ_THREADS) sz_count_kernel(const SerializeParams p) {
+__global__ void __launch_bounds__(TAPE_THREADS) sz_count_kernel(const SerializeParams p) {
     const uint64_t base = (uint64_t)blockIdx.x * SZ_TILE + (uint64_t)threadIdx.x * SZ_ROUNDS;
     uint64_t w[SZ_ROUNDS];
-    HAgg pre = sz_load(p, base, w);
+    HAgg pre = tape_heads(p.t.tape, p.t.n, p.h_tile_pre, p.h_grp_pre, base, w);
     SzSum s{0, 0, 0};
     bool bad = false;
 #pragma unroll
     for (int j = 0; j < SZ_ROUNDS; j++) {
-        if (base + j >= p.n) break;
+        if (base + j >= p.t.n) break;
         if (hagg_out(pre, 1)) {
             uint32_t tag, vals, str;
             bad |= !sz_item(p, base + j, w[j], tag, vals, str);
@@ -154,20 +135,20 @@ __global__ void __launch_bounds__(MJ_THREADS) sz_count_kernel(const SerializePar
 }
 
 // KS2: spos[k] = tape index of string k
-__global__ void __launch_bounds__(MJ_THREADS) sz_index_kernel(const SerializeParams p) {
+__global__ void __launch_bounds__(TAPE_THREADS) sz_index_kernel(const SerializeParams p) {
     const uint64_t base = (uint64_t)blockIdx.x * SZ_TILE + (uint64_t)threadIdx.x * SZ_ROUNDS;
     uint64_t w[SZ_ROUNDS];
-    HAgg pre = sz_load(p, base, w);
+    HAgg pre = tape_heads(p.t.tape, p.t.n, p.h_tile_pre, p.h_grp_pre, base, w);
     uint32_t str = 0;
     bool head[SZ_ROUNDS];
 #pragma unroll
     for (int j = 0; j < SZ_ROUNDS; j++) {
-        head[j] = base + j < p.n && hagg_out(pre, 1);
+        head[j] = base + j < p.t.n && hagg_out(pre, 1);
         str += head[j] && (w[j] >> 56) == '"';
-        if (base + j < p.n) pre = agg_combine(pre, mj_word_agg(w[j], base + j));
+        if (base + j < p.t.n) pre = agg_combine(pre, mj_word_agg(w[j], base + j));
     }
     SzSum total;
-    uint64_t k = p.c_grp_pre[blockIdx.x >> 10].strs + p.c_tile_pre[blockIdx.x].strs + block_exclusive_scan(SzSum{0, 0, str}, total).strs;
+    uint64_t k = tile_prefix(p.c_tile_pre, p.c_grp_pre, blockIdx.x).strs + block_exclusive_scan(SzSum{0, 0, str}, total).strs;
 #pragma unroll
     for (int j = 0; j < SZ_ROUNDS; j++)
         if (head[j] && (w[j] >> 56) == '"') p.spos[k++] = (uint32_t)(base + j);
@@ -176,9 +157,8 @@ __global__ void __launch_bounds__(MJ_THREADS) sz_index_kernel(const SerializePar
 // the bytes of string k (checked by KS1)
 __device__ __forceinline__ const uint8_t* sz_str(const SerializeParams& p, uint64_t k, uint64_t& len) {
     const uint32_t i = p.spos[k];
-    const uint64_t v = p.tape[i] & MJ_VALUE_MASK;
-    len = p.tape[i + 1];
-    return (v & MJ_STRINGBUFBIT) ? p.strings + (v & (MJ_STRINGBUFBIT - 1)) : p.msg + v;
+    len = p.t.tape[i + 1];
+    return tape_string_ptr(p.t, p.t.tape[i]);
 }
 
 __host__ __device__ __forceinline__ uint64_t sz_mix(uint64_t x) {  // splitmix64's finalizer: a bijection
@@ -278,7 +258,7 @@ __global__ void __launch_bounds__(SZ_OTHREADS) sz_resolve_kernel(const Serialize
 // KS5: bytes of the distinct strings per tile of SZ_OTILE ordinals
 __device__ __forceinline__ uint64_t sz_distinct_len(const SerializeParams& p, uint64_t k) {
     if (k >= p.m || p.rep[k] != k) return 0;
-    return p.tape[p.spos[k] + 1];
+    return p.t.tape[p.spos[k] + 1];
 }
 
 __global__ void __launch_bounds__(1024) sz_distinct_kernel(const SerializeParams p) {
@@ -302,7 +282,7 @@ __global__ void __launch_bounds__(1024) sz_message_kernel(const SerializeParams 
         s += len[j];
     }
     MSum total;
-    uint64_t off = p.d_grp_pre[blockIdx.x >> 10].v + p.d_tile_pre[blockIdx.x].v + block_exclusive_scan(MSum{s}, total).v;
+    uint64_t off = tile_prefix(p.d_tile_pre, p.d_grp_pre, blockIdx.x).v + block_exclusive_scan(MSum{s}, total).v;
 #pragma unroll
     for (int j = 0; j < 4; j++) {
         const bool d = base + j < p.m && p.rep[base + j] == base + j;
@@ -328,15 +308,15 @@ __device__ __forceinline__ void sz_put64(uint8_t* o, uint64_t v) {
 }
 
 // KS7: one tag byte per head word and its values
-__global__ void __launch_bounds__(MJ_THREADS) sz_emit_kernel(const SerializeParams p) {
+__global__ void __launch_bounds__(TAPE_THREADS) sz_emit_kernel(const SerializeParams p) {
     const uint64_t base = (uint64_t)blockIdx.x * SZ_TILE + (uint64_t)threadIdx.x * SZ_ROUNDS;
     uint64_t w[SZ_ROUNDS];
-    HAgg pre = sz_load(p, base, w);
+    HAgg pre = tape_heads(p.t.tape, p.t.n, p.h_tile_pre, p.h_grp_pre, base, w);
     bool head[SZ_ROUNDS];
     SzSum s{0, 0, 0};
 #pragma unroll
     for (int j = 0; j < SZ_ROUNDS; j++) {
-        head[j] = base + j < p.n && hagg_out(pre, 1);
+        head[j] = base + j < p.t.n && hagg_out(pre, 1);
         if (head[j]) {
             uint32_t tag, vals, str;
             sz_item(p, base + j, w[j], tag, vals, str);
@@ -344,11 +324,11 @@ __global__ void __launch_bounds__(MJ_THREADS) sz_emit_kernel(const SerializePara
             s.vals += vals;
             s.strs += str;
         }
-        if (base + j < p.n) pre = agg_combine(pre, mj_word_agg(w[j], base + j));
+        if (base + j < p.t.n) pre = agg_combine(pre, mj_word_agg(w[j], base + j));
     }
     SzSum total;
     const SzSum ex = block_exclusive_scan(s, total);
-    SzSum at = agg_combine(agg_combine(p.c_grp_pre[blockIdx.x >> 10], p.c_tile_pre[blockIdx.x]), ex);
+    SzSum at = agg_combine(tile_prefix(p.c_tile_pre, p.c_grp_pre, blockIdx.x), ex);
 #pragma unroll
     for (int j = 0; j < SZ_ROUNDS; j++) {
         if (!head[j]) continue;
@@ -360,11 +340,11 @@ __global__ void __launch_bounds__(MJ_THREADS) sz_emit_kernel(const SerializePara
         switch (tag) {
         case '"':
             sz_put64(o, p.moff[p.rep[at.strs]]);
-            sz_put64(o + 8, p.tape[i + 1]);
+            sz_put64(o + 8, p.t.tape[i + 1]);
             break;
-        case 'e': sz_put64(o, w[j]); sz_put64(o + 8, p.tape[i + 1]); break;
-        case 'l': case 'u': case 'd': sz_put64(o, p.tape[i + 1]); break;
-        case '{': case '[': case 'r': sz_put64(o, (w[j] & MJ_VALUE_MASK) - i); break;
+        case 'e': sz_put64(o, w[j]); sz_put64(o + 8, p.t.tape[i + 1]); break;
+        case 'l': case 'u': case 'd': sz_put64(o, p.t.tape[i + 1]); break;
+        case '{': case '[': case 'r': sz_put64(o, (w[j] & TAPE_VALUE_MASK) - i); break;
         default: break;
         }
         at.tags++;
@@ -525,7 +505,7 @@ __device__ __forceinline__ DzAgg dz_load(const DeserializeParams& p, uint64_t ba
         if (threadIdx.x == 0) p.tile[blockIdx.x] = total;
         return s;
     }
-    return agg_combine(agg_combine(p.grp_pre[blockIdx.x >> 10], p.tile_pre[blockIdx.x]), ex);
+    return agg_combine(tile_prefix(p.tile_pre, p.grp_pre, blockIdx.x), ex);
 }
 
 // KD1: per-tile aggregates; unknown tags

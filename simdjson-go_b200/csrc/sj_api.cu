@@ -22,6 +22,7 @@
 #include "stage1.cuh"
 #include "stage2_stream.cuh"
 #include "stage2.cuh"
+#include "tape.cuh"
 #include "consume.cuh"
 #include "find.cuh"
 #include "marshal.cuh"
@@ -209,10 +210,9 @@ extern "C" void sj_ctx_destroy(sj_ctx* c) {
     cudaSetDevice(c->device);
     if (c->stream) cudaStreamSynchronize(c->stream);
     exchange_release(c);
-    DevBuf* bufs[] = {&c->msg,     &c->idx,     &c->desc,    &c->result,   &c->s2a,      &c->s2b,      &c->s2c,
-                      &c->tape,    &c->strings, &c->test_in, &c->test_out, &c->test_aux, &c->tc_small, &c->tc_roots,
-                      &c->tc_scan, &c->fd_small, &c->fd,     &c->fd_out,   &c->mj,       &c->mj_out,   &c->sz,
-                      &c->sz_tab,  &c->sz_out};
+    DevBuf* bufs[] = {&c->msg,     &c->idx,      &c->desc,     &c->result, &c->s2a,     &c->s2b,    &c->s2c,
+                      &c->tape,    &c->strings,  &c->test_in,  &c->test_out, &c->test_aux, &c->args, &c->scratch,
+                      &c->sz_tab,  &c->tc_roots, &c->tc_scan,  &c->staging};
     for (DevBuf* b : bufs) b->release();
     if (c->host_result) cudaFreeHost(c->host_result);
     free(c->pending);
@@ -539,6 +539,7 @@ extern "C" int sj_test_flatten_bits(sj_ctx* c, const uint64_t* masks, size_t nma
 
 #include "sj_exchange.inl"
 #include "sj_parse.inl"
+#include "sj_tape.inl"
 #include "sj_consume.inl"
 #include "sj_marshal.inl"
 #include "sj_find.inl"

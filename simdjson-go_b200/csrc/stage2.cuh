@@ -22,7 +22,7 @@
 
 namespace sj {
 
-// structural types, the grammar (transition_ok) and STRINGBUFBIT live in s2s_core.h, the atom and escape tables
+// structural types and the grammar (transition_ok) live in s2s_core.h, STRINGBUFBIT and the atom and escape tables
 // (structural_or_ws_or_nul, digit_to_val, escape_map) in bits.h: both are shared with the streaming kernels
 constexpr uint32_t AUX_COPY = 0x80000000u;              // string goes to the string buffer
 constexpr uint32_t AUX_ESC = 0x40000000u;               // string contains escapes (source length != unescaped length)

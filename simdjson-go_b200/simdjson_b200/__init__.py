@@ -177,13 +177,19 @@ class Context:
     def parse_marshal(self, msg, ndjson=False, copy_strings=True):
         """parseMessage + Iter.MarshalJSON (parsed_json.go:394) with the tape left in HBM: (rc, JSON text bytes).  Only
         the text is copied back; on a parse error the text is b""."""
+        # compact text is rarely longer than its input
+        return self._parse_to_bytes(self.L.sj_parse_marshal, msg, ndjson, copy_strings, lambda size: size + 64)
+
+    def _parse_to_bytes(self, fn, msg, ndjson, copy_strings, guess):
+        """fn (sj_parse_marshal / sj_parse_serialize) into a buffer of guess(input bytes), else once more at the exact
+        size: (rc, output bytes), b"" on a parse error"""
         m = _as_u8(msg)
         flags = (FLAG_NDJSON if ndjson else 0) | (FLAG_COPY_STRINGS if copy_strings else 0)
         n = C.c_size_t(0)
-        cap = m.size + 64  # compact text is rarely longer than its input; else once more at the exact size
+        cap = guess(m.size)
         for _ in range(2):
             out = np.empty(max(cap, 1), dtype=np.uint8)
-            rc = self.L.sj_parse_marshal(self.h, _addr(m) if m.size else None, m.size, flags, _addr(out), cap, C.byref(n))
+            rc = fn(self.h, _addr(m) if m.size else None, m.size, flags, _addr(out), cap, C.byref(n))
             if rc != ERR_CAPACITY:
                 break
             cap = n.value
@@ -199,12 +205,8 @@ class Context:
         Returns (rc, length of the text, the uint8 tensor view holding it); rc is SJ_ERR_CAPACITY when `out` is too small
         (the length is still exact) and SJ_ERR_ARGUMENT for a malformed tape."""
         import torch
-
-        def ptr_len(t):
-            return (t.data_ptr(), t.numel()) if t is not None and t.numel() else (None, 0)
-
-        sp, sl = ptr_len(strings)
-        mp, ml = ptr_len(message)
+        sp, sl = _ptr_len(strings)
+        mp, ml = _ptr_len(message)
         n = C.c_size_t(0)
         if out is None:
             rc = self.L.sj_marshal_device(self.h, mp, ml, tape.data_ptr(), tape.numel(), sp, sl, None, 0, C.byref(n))
@@ -219,21 +221,8 @@ class Context:
     def parse_serialize(self, msg, ndjson=False, copy_strings=True):
         """parseMessage + Serializer.Serialize (parsed_serialize.go:200) with the tape left in HBM: (rc, stream bytes).
         Only the stream is copied back; on a parse error it is b""."""
-        m = _as_u8(msg)
-        flags = (FLAG_NDJSON if ndjson else 0) | (FLAG_COPY_STRINGS if copy_strings else 0)
-        n = C.c_size_t(0)
-        cap = 2 * m.size + 64  # tags + values are about 1.5x the input at most for typical JSON; else once more at the exact size
-        for _ in range(2):
-            out = np.empty(max(cap, 1), dtype=np.uint8)
-            rc = self.L.sj_parse_serialize(self.h, _addr(m) if m.size else None, m.size, flags, _addr(out), cap, C.byref(n))
-            if rc != ERR_CAPACITY:
-                break
-            cap = n.value
-        if rc in (ERR_STAGE1, ERR_STAGE2):
-            return rc, b""
-        if rc != OK:
-            raise SjError(rc)
-        return rc, out[:n.value].tobytes()
+        # tags + values are about 1.5x the input at most for typical JSON
+        return self._parse_to_bytes(self.L.sj_parse_serialize, msg, ndjson, copy_strings, lambda size: 2 * size + 64)
 
     def serialize_device(self, tape, strings=None, message=None, out=None):
         """Serializer.Serialize of a tape already on this context's device, arguments as marshal_device.  Returns (rc,

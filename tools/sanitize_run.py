@@ -45,6 +45,40 @@ same(pk[:120000 if quick else len(pk)].rsplit(b"\n", 1)[0], ndjson=True)
 nd, _ = tricky_ndjson()
 same(nd, ndjson=True)
 assert ctx.parse_count_where(nd, b"Make", b"HOND")[0] == 0
+# the tape consumers' device entry points (tape.cuh) on the context's own tape (stage 2's root list) and on a copy of it
+# (a foreign tape: KM1 + KC1a / KC1b)
+import ctypes as C
+
+import torch
+
+from tests import find_oracle as fo
+from tests.marshal_oracle import marshal
+from tests.serialize_oracle import serialize
+
+small = b"\n".join(pk.split(b"\n")[:40])
+rc_o, tape_o, str_o, (off_o, len_o) = o.parse(small, ndjson=True)
+d_msg = torch.full((len(small) + 4096,), 0x20, dtype=torch.uint8, device="cuda")
+d_msg[:len(small)].copy_(torch.frombuffer(bytearray(small), dtype=torch.uint8))
+tcap, scap, tl, sl = C.c_size_t(0), C.c_size_t(0), C.c_size_t(0), C.c_size_t(0)
+ctx.L.sj_bounds(len(small), C.byref(tcap), C.byref(scap))
+d_tape = torch.empty(tcap.value, dtype=torch.int64, device="cuda")
+d_str = torch.empty(scap.value, dtype=torch.uint8, device="cuda")
+assert ctx.L.sj_parse_device(ctx.h, d_msg.data_ptr(), len(small), 3, d_tape.data_ptr(), d_tape.numel(), C.byref(tl),
+                             d_str.data_ptr(), d_str.numel(), C.byref(sl)) == 0
+own, strs, msg = d_tape[:tl.value], d_str[:sl.value], d_msg[:len(small)]
+paths, kinds = [[b"Make"], [b"Fine"]], [fo.STRING, fo.ELEMENT]
+win = small[off_o:off_o + len_o]
+want_text, want_stream = marshal(tape_o, str_o, win), serialize(tape_o, str_o, win)
+for tape in (own, own.clone()):
+    rc, rows, cols = ctx.find_device(tape, strs, msg, paths, kinds)
+    assert rc == 0 and rows == 40, (rc, rows)
+    rc, _, text = ctx.marshal_device(tape, strs, msg)
+    assert rc == 0 and text.cpu().numpy().tobytes() == want_text
+    rc, _, stream = ctx.serialize_device(tape, strs, msg)
+    assert rc == 0 and stream.cpu().numpy().tobytes() == want_stream
+    rc, sizes, (t2, s2, m2) = ctx.deserialize_device(stream)
+    assert rc == 0 and ctx.marshal_device(t2[:sizes[0]], s2[:sizes[1]], m2[:sizes[2]])[2].cpu().numpy().tobytes() == want_text
+    n += 1
 # carries across slab / tile edges, long strings (warp-cooperative paths), dense brackets, number-heavy
 g = (__import__("ctypes").c_uint32 * 4)()
 ctx.L.sj_test_geometry(g)
@@ -59,10 +93,7 @@ same(b"[" + b",".join(b"%d.%de%d" % (i, i * 7919 % 100000, i % 30 - 15) for i in
 same(b'{"a":tru}')
 same(b'["abc\\q"]')
 # the sharded ParseND with the exchange kernel over peer memory (exchange.cuh): two host threads = two ranks on this GPU
-import ctypes as C
 import threading
-
-import torch
 
 from simdjson_b200.parallel import ShardedParse, split_at_newlines, trimmed_window
 
