@@ -13,6 +13,54 @@
 
 namespace sj {
 
+// K2r's section probe (tools/k2r_probe.py builds it; the product build does not define SJ_K2R_PROBE): a clock64()
+// stamp at each section boundary of the slab loop, the per-slab sums added into sj_k2r_probe_cycles once per slab.
+// The stamps cost time themselves, so the sums are for shares, not for K2r's time.
+enum : uint32_t {
+    K2R_PROLOGUE,   // slab prologue: carries, prefixes, pre-types
+    K2R_IMAGE,      // image pipeline: issue the next step, wait for this one
+    K2R_CLASSIFY,   // classify, escape starts, quote mask, escapes
+    K2R_EVENTS,     // step_events and the scans of the step
+    K2R_STRINGS,    // Strings.B compaction and copy-out
+    K2R_GRAMMAR,    // pre-types and the grammar masks
+    K2R_EMIT,       // emission loops
+    K2R_LINK,       // in-step links and tape copy-out
+    K2R_SECTIONS
+};
+#if defined(SJ_K2R_PROBE) && defined(__CUDACC__)
+__device__ unsigned long long sj_k2r_probe_cycles[K2R_SECTIONS];
+#endif
+#if defined(SJ_K2R_PROBE) && defined(__CUDA_ARCH__)
+// (lane k keeps the sum of section k: three registers in all)
+#define K2R_PROBE_START        \
+    uint32_t probe_acc = 0;    \
+    long long probe_t = clock64();
+#define K2R_PROBE(sec)                                        \
+    do {                                                      \
+        __syncwarp();                                         \
+        const long long t_ = clock64();                       \
+        if (lane == (sec)) probe_acc += (uint32_t)(t_ - probe_t); \
+        probe_t = t_;                                         \
+    } while (0)
+#define K2R_PROBE_FLUSH                                                                          \
+    do {                                                                                         \
+        if (lane < K2R_SECTIONS) atomicAdd(&sj_k2r_probe_cycles[lane], (unsigned long long)probe_acc); \
+    } while (0)
+#else
+#define K2R_PROBE_START
+#define K2R_PROBE(sec) \
+    do {               \
+    } while (0)
+#define K2R_PROBE_FLUSH \
+    do {                \
+    } while (0)
+#endif
+
+template <bool B>
+struct BoolC {
+    static constexpr bool value = B;
+};
+
 // original message bytes: the slab image in shared memory where it covers the position, global memory elsewhere,
 // 0 beyond the end of the message (the reference reads zero padding there, stage2...go:75-86)
 struct MsgReader {
@@ -382,6 +430,7 @@ template <class W, bool EMIT>
 SJ_HD void s2s_slab(W& wp, const S2sParams& p, uint32_t slab, const S2sWarpMem& sm, uint32_t& cur, uint32_t next_slab) {
     const uint32_t lane = wp.lane();
     const uint32_t lt = (1u << lane) - 1u;
+    K2R_PROBE_START
     const uint64_t slab_start = (uint64_t)slab * S2S_SLAB_BYTES;
     const uint64_t slab_end = slab_start + S2S_SLAB_BYTES < p.len ? slab_start + S2S_SLAB_BYTES : p.len;
     const GlobalReader g{p.msg, p.len};
@@ -447,6 +496,7 @@ SJ_HD void s2s_slab(W& wp, const S2sParams& p, uint32_t slab, const S2sWarpMem& 
         }
     }
 
+    K2R_PROBE(K2R_PROLOGUE);
     for (uint32_t s = 0; s < S2S_STEPS; s++) {
         const uint64_t step_start = slab_start + (uint64_t)s * S2S_STEP_BYTES;
         if (step_start >= p.len) break;  // warp-uniform
@@ -462,6 +512,7 @@ SJ_HD void s2s_slab(W& wp, const S2sParams& p, uint32_t slab, const S2sWarpMem& 
             wp.async_wait_prev();
             wp.sync();
         }
+        K2R_PROBE(K2R_IMAGE);
         const uint8_t* sbase = sm.src + cur * S2S_STEP_BYTES;
         cur ^= 1u;
         rd.src = sbase;
@@ -626,6 +677,7 @@ SJ_HD void s2s_slab(W& wp, const S2sParams& p, uint32_t slab, const S2sWarpMem& 
             }
         }
 
+        K2R_PROBE(K2R_CLASSIFY);
         // ---------------- E: structurals (finalize_structurals_amd64.s:19-36), events, counts ----------------
         const StepEvents ev = step_events(wp, m, qm, qb, K, p.ndjson, ppc, recc);
         const uint64_t closeq = ev.closeq, V = ev.V, NLS = ev.NLS, EV = ev.EV, recst = ev.recst;
@@ -687,16 +739,23 @@ SJ_HD void s2s_slab(W& wp, const S2sParams& p, uint32_t slab, const S2sWarpMem& 
             }
         }
 
+        K2R_PROBE(K2R_EVENTS);
         // ---------------- Strings.B: byte compaction of the step into the staging area ----------------
         const uint32_t str_base = run.str;                 // offset of the step's bytes in Strings.B
         const uint32_t shift = (uint32_t)(reinterpret_cast<uintptr_t>(p.strings + str_base) & 15u);  // staging keeps the destination's 16-byte phase
         if (k_step) {                                      // warp-uniform
+            // Every staging word in [shift / 4, (shift + k_step - 1) / 4] is stored exactly once, with a plain store, by
+            // the lane that holds its first output byte: whole words as they fill, and the SEAM word a lane's bytes end
+            // in after the lanes above have handed it the bytes they put into it.  Those lanes start their output in
+            // the middle of the word (o & 3 != 0) and feed their first word's bytes (`feed`) instead of storing it; each
+            // gives at least one byte, so at most three of them share the word with its owner.  The bytes in front of
+            // `shift` and behind the step's last byte are never read.
             uint32_t* st32 = reinterpret_cast<uint32_t*>(sm.sstage);
-            for (uint32_t i = lane; i < S2S_SSTAGE_BYTES / 16; i += 32) reinterpret_cast<V16*>(sm.sstage)[i] = V16{0, 0, 0, 0};
-            wp.sync();
+            const uint32_t o = shift + k_ex;               // first output byte of the lane
+            const uint32_t first = o >> 2;
+            const bool feeds = (o & 3u) != 0 && o != shift;  // a lane below holds the first byte of the lane's first word
+            uint32_t feed = 0, seam = 0, seam_at = ~0u;
             if (k_lane) {
-                const uint32_t o = shift + k_ex;           // first output byte of the lane
-                const uint32_t first = o >> 2;
                 uint32_t ptr = first, fill = o & 3u, lo = 0;
                 const uint32_t Klo = (uint32_t)K, Khi = (uint32_t)(K >> 32);
 #pragma unroll
@@ -709,8 +768,8 @@ SJ_HD void s2s_slab(W& wp, const S2sParams& p, uint32_t slab, const S2sWarpMem& 
                     const uint32_t hi = pi::funnel_l(cw, 0, 8 * fill);
                     fill += cnt;
                     if (fill >= 4) {
-                        if (ptr == first)
-                            wp.atomic_or_shared(st32 + ptr, lo);  // shared with the lane below
+                        if (ptr == first && feeds)
+                            feed = lo;
                         else
                             st32[ptr] = lo;
                         ptr++;
@@ -718,9 +777,23 @@ SJ_HD void s2s_slab(W& wp, const S2sParams& p, uint32_t slab, const S2sWarpMem& 
                         fill -= 4;
                     }
                 }
-                if (fill) wp.atomic_or_shared(st32 + ptr, lo);  // shared with the lane above
+                if (fill) {
+                    if (ptr == first && feeds)
+                        feed = lo;
+                    else
+                        seam = lo, seam_at = ptr;
+                }
             }
-            wp.sync();
+            // the next three lanes with output bytes: those whose first word is the seam word feed it
+            uint32_t above = wp.ballot(k_lane != 0) & ~((2u << lane) - 1u);
+#pragma unroll
+            for (int j = 0; j < 3; j++) {
+                const uint32_t src = above ? (uint32_t)pi::ctz32(above) : lane;
+                const uint32_t f_src = wp.shfl(first, src), v_src = wp.shfl(feed, src);
+                if (above && f_src == seam_at) seam |= v_src;
+                above &= above - 1u;
+            }
+            if (seam_at != ~0u) st32[seam_at] = seam;
             wp.sync();
             // copy-out: head and tail bytes one by one, the 16-byte aligned middle as vectors
             {
@@ -737,6 +810,7 @@ SJ_HD void s2s_slab(W& wp, const S2sParams& p, uint32_t slab, const S2sWarpMem& 
             }
         }
 
+        K2R_PROBE(K2R_STRINGS);
         // ---------------- the lane's events, in order ----------------
         // The step's tape words [slot0, slot0 + w_step) go to the tape-staging area at the destination's 32-byte phase
         // and out in whole sectors behind the loops; scattered 8-byte stores straight to the tape would each land on a
@@ -808,12 +882,14 @@ SJ_HD void s2s_slab(W& wp, const S2sParams& p, uint32_t slab, const S2sWarpMem& 
                 BADR = EV & ~OKR, BADO = EV & ~OKO, BADA = EV & ~OKA;
             }
             if (V & ~m.numc & ~m.atomc) err = 1;  // a value that starts with neither a digit, '-' nor t / f / n
+            K2R_PROBE(K2R_GRAMMAR);
 
             // ---- emission: one uniform loop per class of event; the tape slot of an event = words of the events below
             // it.  The block is handled as two 32-bit halves so that every mask operation is a single-register one. ----
             const uint64_t W1 = BRK | ATOM, W2 = closeq | NUM;  // one-word / two-word events
             const uint64_t OPENS = O1 | O2;
             const uint32_t lane_str = str_base + k_ex;          // Strings.B offset of the lane's first kept byte
+            const uint64_t str_tag = (uint64_t)'"' << 56, str_buf = STRINGBUFBIT + out_str_base;
             uint32_t words_b = slot0 + w_ex;                     // tape slot of the half's first word
             uint32_t kb_b = run.brk + b_ex, rec_b = run.rec + r_ex, num_b = run.num + n_ex, rank_b = 0;
             int32_t depth_b = run.depth + d_ex;
@@ -829,69 +905,89 @@ SJ_HD void s2s_slab(W& wp, const S2sParams& p, uint32_t slab, const S2sWarpMem& 
                 const uint64_t half_pos = block_pos + 32 * h;
                 // record boundaries (root close + root open: the words themselves are written by K2f, or below)
                 for (uint32_t mm = rs; mm; mm &= mm - 1) {
-                    const uint32_t lo = (1u << pi::ctz32(mm)) - 1u;
+                    const uint32_t lo = (mm & (0u - mm)) - 1u;
                     const uint32_t below = pi::popc32(rs & lo);
                     const uint32_t open = words_b + pi::popc32(w1 & lo) + 2 * (pi::popc32(w2 & lo) + below) + 1;
                     p.rootpos[rec_b + below + 1] = open;
                     if (link_r) lst[S2S_LINK_BRK_CAP + rec_b - run.rec + below] = open;
                 }
-                // brackets: records for the scope matching, the tape word, the grammar verdict of the segment they end
-                {
-                    uint32_t prevm = 0;  // bits up to and including the previous bracket of the half
-                    for (uint32_t mm = brk; mm; mm &= mm - 1) {
-                        const uint32_t j = pi::ctz32(mm), bit = 1u << j, lo = bit - 1u, upto = lo | bit;
-                        const uint32_t slot = words_b + pi::popc32(w1 & lo) + 2 * (pi::popc32(w2 & lo) + pi::popc32(rs & upto));
-                        const uint32_t kb = kb_b + pi::popc32(brk & lo);
-                        const bool curly = (cur & bit) != 0, opening = (opn & bit) != 0;
-                        const int32_t dep = depth_b + (int32_t)pi::popc32(opn & lo) - (int32_t)pi::popc32(brk & ~opn & lo);
-                        const uint32_t kind = opening ? (curly ? T_OBJ_OPEN : T_ARR_OPEN) : (curly ? T_OBJ_CLOSE : T_ARR_CLOSE);
-                        p.brk_tp[kb] = slot;
-                        p.brk_depth[kb] = dep;
-                        if (link_b)  // staging index (10 bits) | kind (3) | depth in front relative to the step's, + 4096 (13)
-                            lst[kb - run.brk] = (slot - sslot) | (kind << 10) | ((uint32_t)(dep - run.depth + 4096) << 13);
-                        else
-                            p.brk_kind[kb] = (uint8_t)kind;
-                        put(slot, (uint64_t)((opening ? 0x5bu : 0x5du) | (curly ? 0x20u : 0u)) << 56);  // payload: cross-linked below or by K2e
-                        const uint32_t seg = upto & ~prevm;
-                        const uint32_t bad = segbad | ((bdr & seg) ? 1u : 0u) | ((bdo & seg) ? 2u : 0u) | ((bda & seg) ? 4u : 0u);
-                        if (bad) wp.atomic_and(p.segmask + (kb >> 2), ~(bad << (8 * (kb & 3))));
-                        segbad = 0;
-                        prevm = upto;
+                // The tape slot of an event at bit j: words_b + one word per w1 event and two per w2 event below it + two
+                // per record start below it (for brackets, numbers and atoms: at or below it -- their root words come
+                // first).  A record start sits on stage 1's structural -- a bracket, an opening quote or a value start --
+                // so it shares a bit with w2 only where a record starts with a number.  A lane whose half has no such bit
+                // (FOLD) counts the record starts with w2 (w2r): two popcounts per slot instead of three.  On a bracket
+                // or an atom w2 has no bit, so w2r up to and including the event's own bit counts its record start; on
+                // a number rs has none.
+                const uint32_t w2r = w2 | rs;
+                const uint32_t str_lane = lane_str + rank_b;  // Strings.B offset of the half's first kept byte
+                auto events = [&](auto fold) {
+                    constexpr bool FOLD = decltype(fold)::value;
+                    // brackets: records for the scope matching, the tape word, the grammar verdict of the segment they end
+                    {
+                        uint32_t prevm = 0;  // bits up to and including the previous bracket of the half
+                        for (uint32_t mm = brk; mm; mm &= mm - 1) {
+                            const uint32_t bit = mm & (0u - mm), lo = bit - 1u, upto = lo | bit;
+                            const uint32_t slot = FOLD ? words_b + pi::popc32(w1 & lo) + 2 * pi::popc32(w2r & upto)
+                                                       : words_b + pi::popc32(w1 & lo) + 2 * (pi::popc32(w2 & lo) + pi::popc32(rs & upto));
+                            const uint32_t nb = pi::popc32(brk & lo), kb = kb_b + nb;
+                            const bool curly = (cur & bit) != 0, opening = (opn & bit) != 0;
+                            const int32_t dep = depth_b + 2 * (int32_t)pi::popc32(opn & lo) - (int32_t)nb;  // opens - closes below
+                            const uint32_t kind = opening ? (curly ? T_OBJ_OPEN : T_ARR_OPEN) : (curly ? T_OBJ_CLOSE : T_ARR_CLOSE);
+                            p.brk_tp[kb] = slot;
+                            p.brk_depth[kb] = dep;
+                            if (link_b)  // staging index (10 bits) | kind (3) | depth in front relative to the step's, + 4096 (13)
+                                lst[kb - run.brk] = (slot - sslot) | (kind << 10) | ((uint32_t)(dep - run.depth + 4096) << 13);
+                            else
+                                p.brk_kind[kb] = (uint8_t)kind;
+                            put(slot, (uint64_t)((opening ? 0x5bu : 0x5du) | (curly ? 0x20u : 0u)) << 56);  // payload: cross-linked below or by K2e
+                            const uint32_t seg = upto & ~prevm;
+                            const uint32_t bad = segbad | ((bdr & seg) ? 1u : 0u) | ((bdo & seg) ? 2u : 0u) | ((bda & seg) ? 4u : 0u);
+                            if (bad) wp.atomic_and(p.segmask + (kb >> 2), ~(bad << (8 * (kb & 3))));
+                            segbad = 0;
+                            prevm = upto;
+                        }
+                        const uint32_t seg = ~prevm;  // behind the half's last bracket: the segment goes on
+                        segbad |= ((bdr & seg) ? 1u : 0u) | ((bdo & seg) ? 2u : 0u) | ((bda & seg) ? 4u : 0u);
                     }
-                    const uint32_t seg = ~prevm;  // behind the half's last bracket: the segment goes on
-                    segbad |= ((bdr & seg) ? 1u : 0u) | ((bdo & seg) ? 2u : 0u) | ((bda & seg) ? 4u : 0u);
-                }
-                // strings, at their closing quote (stage2...go:72-113)
-                for (uint32_t mm = cq; mm; mm &= mm - 1) {
-                    const uint32_t lo = (1u << pi::ctz32(mm)) - 1u;
-                    const uint32_t slot = words_b + pi::popc32(w1 & lo) + 2 * (pi::popc32(w2 & lo) + pi::popc32(rs & lo));
-                    const uint32_t kbelow = pi::popc32(kk & lo);
-                    const uint32_t lower = qq & lo;  // the opening quote is the highest quote below, if it is in this half
-                    const uint32_t dl = lower ? pi::popc32(kk & lo & ~((1u << (31 - pi::clz32(lower))) - 1u)) : pre_dl + kbelow;
-                    put(slot, ((uint64_t)'"' << 56) | (STRINGBUFBIT + out_str_base + (uint64_t)(lane_str + rank_b + kbelow - dl)));
-                    put(slot + 1, dl);
-                }
-                // numbers: parsed by K2h from the list
-                for (uint32_t mm = num; mm; mm &= mm - 1) {
-                    const uint32_t j = pi::ctz32(mm), bit = 1u << j, lo = bit - 1u;
-                    NumEntry ne;
-                    ne.pos = (uint32_t)(half_pos + j);
-                    ne.slot = words_b + pi::popc32(w1 & lo) + 2 * (pi::popc32(w2 & lo) + pi::popc32(rs & (lo | bit)));
-                    p.numlist[num_b + pi::popc32(num & lo)] = ne;
-                }
-                // atoms
-                for (uint32_t mm = atm; mm; mm &= mm - 1) {
-                    const uint32_t j = pi::ctz32(mm), bit = 1u << j, lo = bit - 1u;
-                    const uint32_t slot = words_b + pi::popc32(w1 & lo) + 2 * (pi::popc32(w2 & lo) + pi::popc32(rs & (lo | bit)));
-                    uint32_t ch;
-                    bool ok;
-                    if (!atom_ok_fast(sbase, 64 * lane + 32 * h + j, (uint32_t)(rd.slab_end - rd.slab_start), &ch, &ok)) {
-                        ch = sbase[swz(64 * lane + 32 * h + j)];
-                        ok = atom_ok_p(rd, half_pos + j, p.len, sm.ctab[ch]);
+                    // strings, at their closing quote (stage2...go:72-113)
+                    for (uint32_t mm = cq; mm; mm &= mm - 1) {
+                        const uint32_t lo = (mm & (0u - mm)) - 1u;
+                        const uint32_t slot = FOLD ? words_b + pi::popc32(w1 & lo) + 2 * pi::popc32(w2r & lo)
+                                                   : words_b + pi::popc32(w1 & lo) + 2 * (pi::popc32(w2 & lo) + pi::popc32(rs & lo));
+                        const uint32_t kbelow = pi::popc32(kk & lo);
+                        const uint32_t lower = qq & lo;  // the opening quote is the highest quote below, if it is in this half
+                        const uint32_t dl = lower ? pi::popc32(kk & lo & ~((1u << (31 - pi::clz32(lower))) - 1u)) : pre_dl + kbelow;
+                        put(slot, str_tag | (str_buf + (uint64_t)(str_lane + kbelow - dl)));
+                        put(slot + 1, dl);
                     }
-                    if (!ok) err = 1;
-                    put(slot, (uint64_t)ch << 56);
-                }
+                    // numbers: parsed by K2h from the list
+                    for (uint32_t mm = num; mm; mm &= mm - 1) {
+                        const uint32_t j = pi::ctz32(mm), bit = 1u << j, lo = bit - 1u;
+                        NumEntry ne;
+                        ne.pos = (uint32_t)(half_pos + j);
+                        ne.slot = FOLD ? words_b + pi::popc32(w1 & lo) + 2 * pi::popc32(w2r & lo)
+                                       : words_b + pi::popc32(w1 & lo) + 2 * (pi::popc32(w2 & lo) + pi::popc32(rs & (lo | bit)));
+                        p.numlist[num_b + pi::popc32(num & lo)] = ne;
+                    }
+                    // atoms
+                    for (uint32_t mm = atm; mm; mm &= mm - 1) {
+                        const uint32_t j = pi::ctz32(mm), bit = 1u << j, lo = bit - 1u;
+                        const uint32_t slot = FOLD ? words_b + pi::popc32(w1 & lo) + 2 * pi::popc32(w2r & (lo | bit))
+                                                   : words_b + pi::popc32(w1 & lo) + 2 * (pi::popc32(w2 & lo) + pi::popc32(rs & (lo | bit)));
+                        uint32_t ch;
+                        bool ok;
+                        if (!atom_ok_fast(sbase, 64 * lane + 32 * h + j, (uint32_t)(rd.slab_end - rd.slab_start), &ch, &ok)) {
+                            ch = sbase[swz(64 * lane + 32 * h + j)];
+                            ok = atom_ok_p(rd, half_pos + j, p.len, sm.ctab[ch]);
+                        }
+                        if (!ok) err = 1;
+                        put(slot, (uint64_t)ch << 56);
+                    }
+                };
+                if ((w2 & rs) == 0)  // per lane (no collective inside)
+                    events(BoolC<true>());
+                else
+                    events(BoolC<false>());
                 // totals of the half
                 const uint32_t nk = pi::popc32(kk), nopn = pi::popc32(opn), nbr = pi::popc32(brk);
                 words_b += pi::popc32(w1) + 2 * (pi::popc32(w2) + pi::popc32(rs));
@@ -905,6 +1001,7 @@ SJ_HD void s2s_slab(W& wp, const S2sParams& p, uint32_t slab, const S2sWarpMem& 
             // the segment behind the lane's last bracket goes on in the next lanes
             if (segbad) wp.atomic_and(p.segmask + (kb_b >> 2), ~(segbad << (8 * (kb_b & 3))));
         }
+        K2R_PROBE(K2R_EMIT);
         if (staged) {
             wp.sync();
             if (link_b || link_r) {
@@ -966,6 +1063,7 @@ SJ_HD void s2s_slab(W& wp, const S2sParams& p, uint32_t slab, const S2sWarpMem& 
             }
         }
         wp.sync();  // the staging areas and the escape scratch are reused by the next step
+        K2R_PROBE(K2R_LINK);
         run.w += w_step;
         run.str += k_step;
         run.brk += b_step;
@@ -974,6 +1072,7 @@ SJ_HD void s2s_slab(W& wp, const S2sParams& p, uint32_t slab, const S2sWarpMem& 
         run.num += n_step;
     }
 
+    if (EMIT) K2R_PROBE_FLUSH;
     if (wp.any(err != 0) && lane == 0) wp.atomic_or(p.error, 1u);
     if (EMIT && lane == 0) {  // the counts K2r went by against the ones stage 1 added up for the slab
         const SlabAgg want = agg_combine(start, p.agg[slab]);

@@ -325,6 +325,19 @@ extern "C" int sj_kernel_launches(sj_ctx* c, uint64_t* count) {
     return SJ_OK;
 }
 
+#ifdef SJ_K2R_PROBE
+// K2r's section probe (s2s_slab.h; built by tools/k2r_probe.py only): the cycle sums so far into out[K2R_SECTIONS],
+// then cleared
+extern "C" int sj_k2r_probe_take(sj_ctx* c, unsigned long long* out) {
+    static const unsigned long long zero[K2R_SECTIONS] = {};
+    SJ_CUDA_CHECK(cudaSetDevice(c->device));
+    SJ_CUDA_CHECK(cudaDeviceSynchronize());
+    SJ_CUDA_CHECK(cudaMemcpyFromSymbol(out, sj_k2r_probe_cycles, sizeof(zero)));
+    SJ_CUDA_CHECK(cudaMemcpyToSymbol(sj_k2r_probe_cycles, zero, sizeof(zero)));
+    return SJ_OK;
+}
+#endif
+
 // ---------------------------------------------------------------------------------
 // stage 1
 // ---------------------------------------------------------------------------------
