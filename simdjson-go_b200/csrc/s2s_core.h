@@ -242,6 +242,27 @@ SJ_HD Class64 classify_block2(const uint32_t (&w)[16]) {
     return m;
 }
 
+// Stage 1's parse mode classifies each block once: next to its structurals st ({ } [ ] , :) it keeps two planes of the
+// same transpose, X = brackets | first bytes of numbers and Y = opening brackets | first bytes of atoms.  No structural
+// starts a number or an atom, so st takes them apart again (classes_from_parse_planes).
+struct ParsePlanes {
+    uint32_t x, y;
+};
+SJ_HD ParsePlanes parse_planes(const uint32_t (&p)[8]) {
+    const Half2 m = classify_planes2(p);
+    return ParsePlanes{m.open | m.close | m.numc, m.open | m.atomc};
+}
+// open, close, cc, numc, atomc of a block from st and its X / Y planes (the other members are left 0)
+SJ_HD Class64 classes_from_parse_planes(uint64_t st, uint64_t x, uint64_t y) {
+    Class64 m{};
+    m.open = st & y;
+    m.close = st & x & ~y;
+    m.cc = st & ~x;
+    m.numc = x & ~st;
+    m.atomc = y & ~st;
+    return m;
+}
+
 // Escape STARTS of a block: the backslashes that sit at an even offset inside their run (every second one, beginning
 // with the first).  `first_escaped` = the block's first byte is consumed by an escape that started in front of the
 // block (the carry of find_odd_backslash_sequences_amd64.s:27-58): a run beginning at bit 0 then starts at an odd offset.

@@ -2,7 +2,7 @@
 // stage2_stream.cuh) and for the host emulation (W = FiberWarp, tests/emu/s2s_emu.cpp).  See s2s_core.h for the idea.
 //
 //   s2s_slab<W, false>   counts of the slab -> SlabAgg (the emulator's counting pass; on the device stage 1's parse mode
-//                        counts, with step_events / agg_add_step below)
+//                        counts, with step_events / agg_lane_add / agg_warp_finish below)
 //   s2s_slab<W, true>    K2r: tape words, Strings.B bytes, bracket records, number list, grammar masks
 //
 // W provides: lane(), ballot(bool), any(bool), shfl / shfl_up (uint32_t), reduce_add(uint32_t), sync(),
@@ -332,31 +332,35 @@ SJ_HD StepEvents step_events(W& wp, const Class64& m, uint64_t qm, uint64_t qb, 
     return e;
 }
 
-// The step's counts added to the slab's running totals.  `trail` / `hasq`: bytes behind the slab's last quote so far,
-// and whether it has one; SlabAgg::last is kept by the caller (agg_last_step).
-template <class W>
-SJ_HD void agg_add_step(W& wp, const StepEvents& e, SlabAgg& run, uint32_t& trail, uint32_t& hasq) {
-    const uint32_t lane = wp.lane();
-    run.w += wp.reduce_add(e.w_lane);
-    run.brk += wp.reduce_add(e.n_brk);
-    run.rec += wp.reduce_add(e.n_rec);
-    run.depth += (int32_t)wp.reduce_add(2 * e.n_open + 64 - e.n_brk) - 64 * 32;
-    run.num += wp.reduce_add(e.n_num);
-    const uint32_t k_step = wp.reduce_add(e.k_lane);
-    run.str += k_step;
-    const uint32_t Q = wp.ballot(e.q_lane);
-    if (Q) {
-        const uint32_t top = 31 - pi::clz32(Q);
-        trail = wp.shfl(e.t_lane, top) + wp.reduce_add(lane > top ? e.k_lane : 0u);
-        hasq = 1;
+// The lane's share of the slab's counts, added up over the slab's steps without a collective (agg_lane_add);
+// agg_warp_finish turns the 32 shares into the slab's SlabAgg once per slab.
+struct LaneAgg {
+    uint32_t w, str, brk, rec, num;
+    int32_t depth;
+    uint32_t kstep;  // the lane's Strings.B bytes of step s in bits 8s..8s+7 (at most 64 per step)
+    uint32_t tq;     // Strings.B bytes behind the lane's last real quote so far
+    uint32_t qstep;  // 1 + the step of the lane's last real quote; 0: none yet
+};
+SJ_HD LaneAgg lane_agg_zero() { return LaneAgg{0, 0, 0, 0, 0, 0, 0, 0, 0}; }
+SJ_HD void agg_lane_add(LaneAgg& a, const StepEvents& e, uint32_t s) {
+    a.w += e.w_lane;
+    a.str += e.k_lane;
+    a.brk += e.n_brk;
+    a.rec += e.n_rec;
+    a.num += e.n_num;
+    a.depth += (int32_t)(2 * e.n_open) - (int32_t)e.n_brk;
+    a.kstep |= e.k_lane << (8 * s);
+    if (e.q_lane) {
+        a.tq = e.t_lane;
+        a.qstep = s + 1;
     } else {
-        trail += k_step;
+        a.tq += e.k_lane;
     }
 }
 
-// SlabAgg::last of the step's structurals S, in front of which lie `last`; byte(o) = the step's byte at offset o
+// SlabAgg::last of one step's structurals S alone; byte(o) = the step's byte at offset o
 template <class W, class B>
-SJ_HD uint32_t agg_last_step(W& wp, uint64_t S, uint32_t last, const B& byte) {
+SJ_HD uint32_t last_of_step(W& wp, uint64_t S, const B& byte) {
     const uint32_t lane = wp.lane();
     uint32_t v = 0, n = 0;
     for (uint64_t r = S; r && n < 3; n++) {  // the lane's last three, the last one first
@@ -369,7 +373,41 @@ SJ_HD uint32_t agg_last_step(W& wp, uint64_t S, uint32_t last, const B& byte) {
         const uint32_t o = wp.shfl(v, lane + d < 32 ? lane + d : lane);
         if (lane + d < 32) v = last_combine(v, o);
     }
-    return last_combine(last, wp.shfl(v, 0));
+    return wp.shfl(v, 0);
+}
+
+// The slab's SlabAgg from the lanes' shares and the structurals S[s] of its steps (0 for steps behind the end of the
+// message); byte(s, o) = the byte at offset o of step s.  SlabAgg::last is taken from the last steps that hold a
+// structural, walking back only while fewer than three are found.
+template <class W, class B>
+SJ_HD SlabAgg agg_warp_finish(W& wp, const LaneAgg& a, const uint64_t (&S)[S2S_STEPS], const B& byte) {
+    const uint32_t lane = wp.lane();
+    SlabAgg r;
+    r.w = wp.reduce_add(a.w);
+    r.str = wp.reduce_add(a.str);
+    r.brk = wp.reduce_add(a.brk);
+    r.rec = wp.reduce_add(a.rec);
+    r.num = wp.reduce_add(a.num);
+    r.depth = (int32_t)wp.reduce_add((uint32_t)a.depth);
+    // trail: the Strings.B bytes behind the slab's last real quote, which lies in the top lane among those whose last
+    // quote is in the slab's last step with a quote; every step if the slab has none
+    r.trail = r.str;
+    for (uint32_t s = S2S_STEPS; s >= 1; s--) {
+        const uint32_t Q = wp.ballot(a.qstep == s);
+        if (Q) {  // warp-uniform
+            const uint32_t top = 31 - pi::clz32(Q);
+            const uint32_t from = lane > top ? s - 1 : s;  // the lane's blocks from this step on lie behind the quote
+            uint32_t behind = 0;
+            for (uint32_t t = from; t < S2S_STEPS; t++) behind += (a.kstep >> (8 * t)) & 0xffu;
+            r.trail = TRAIL_HASQ | (wp.shfl(a.tq, top) + wp.reduce_add(lane == top ? 0u : behind));
+            break;
+        }
+    }
+    r.last = 0;
+    for (uint32_t s = S2S_STEPS; s >= 1 && (r.last >> 24) < 3; s--) {
+        if (wp.any(S[s - 1] != 0)) r.last = last_combine(last_of_step(wp, S[s - 1], [&](uint32_t o) { return byte(s - 1, o); }), r.last);
+    }
+    return r;
 }
 
 // Does SlabAgg::last in front of `slab` name the bytes under the last structurals of stage 1's index (p.idx) in front of
@@ -484,7 +522,8 @@ SJ_HD void s2s_slab(W& wp, const S2sParams& p, uint32_t slab, const S2sWarpMem& 
     uint32_t recc = (p.ndjson && !par && slab > 0) ? record_carry_in(wp, g, slab_start, peekc) : 0u;
 
     // ---- running totals of the slab (K2p) / running prefixes (K2r) ----
-    uint32_t trail = 0, hasq = 0;  // K2p: bytes behind the last quote so far
+    LaneAgg la = lane_agg_zero();  // counting pass: the lane's share of the slab's counts
+    uint64_t S_step[S2S_STEPS] = {};  // counting pass: the structurals of each step, for SlabAgg::last
     uint32_t partial = 0;          // K2r: bytes the string that is open at the step start has contributed so far
     uint32_t pr = T_START;         // K2r: refined type of the last event in front of the step
     uint32_t err = 0;
@@ -686,8 +725,8 @@ SJ_HD void s2s_slab(W& wp, const S2sParams& p, uint32_t slab, const S2sWarpMem& 
         const bool q_lane = ev.q_lane;
 
         if (!EMIT) {
-            agg_add_step(wp, ev, run, trail, hasq);
-            run.last = agg_last_step(wp, ev.S, run.last, [&](uint32_t o) { return (uint32_t)sbase[swz(o)]; });
+            agg_lane_add(la, ev, s);
+            S_step[s] = ev.S;
             continue;
         }
 
@@ -1086,9 +1125,9 @@ SJ_HD void s2s_slab(W& wp, const S2sParams& p, uint32_t slab, const S2sWarpMem& 
             if (p.internal) wp.atomic_or(p.internal, 1u);
         }
     }
-    if (!EMIT && lane == 0) {
-        run.trail = (hasq ? TRAIL_HASQ : 0u) | (trail & ~TRAIL_HASQ);
-        p.agg[slab] = run;
+    if (!EMIT) {  // (the step images are gone by now; structurals sit on original message bytes)
+        const SlabAgg a = agg_warp_finish(wp, la, S_step, [&](uint32_t s, uint32_t o) { return g(slab_start + (uint64_t)s * S2S_STEP_BYTES + o); });
+        if (lane == 0) p.agg[slab] = a;
     }
 }
 

@@ -337,6 +337,18 @@ extern "C" int sj_k2r_probe_take(sj_ctx* c, unsigned long long* out) {
     return SJ_OK;
 }
 #endif
+#ifdef SJ_K1_PROBE
+// K1's parse-mode section probe (stage1.cuh; built by tools/k1_probe.py only): the cycle sums so far into
+// out[K1P_SECTIONS], then cleared
+extern "C" int sj_k1_probe_take(sj_ctx* c, unsigned long long* out) {
+    static const unsigned long long zero[K1P_SECTIONS] = {};
+    SJ_CUDA_CHECK(cudaSetDevice(c->device));
+    SJ_CUDA_CHECK(cudaDeviceSynchronize());
+    SJ_CUDA_CHECK(cudaMemcpyFromSymbol(out, sj_k1_probe_cycles, sizeof(zero)));
+    SJ_CUDA_CHECK(cudaMemcpyToSymbol(sj_k1_probe_cycles, zero, sizeof(zero)));
+    return SJ_OK;
+}
+#endif
 
 // ---------------------------------------------------------------------------------
 // stage 1

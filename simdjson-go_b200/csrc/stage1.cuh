@@ -43,6 +43,53 @@ constexpr int S1_TILE_BYTES = S1_WARPS * S1_SLAB_BYTES;  // one look-back per ti
 constexpr int S1_BUFS = 2;
 constexpr size_t S1_SMEM_BYTES = (size_t)S1_BUFS * S1_TILE_BYTES + 64;  // tiles + mbarriers
 
+// K1's parse-mode section probe (tools/k1_probe.py builds it; the product build does not define SJ_K1_PROBE): a
+// clock64() stamp at each section boundary of a worker iteration, each warp's sums added into sj_k1_probe_cycles when it
+// leaves the loop.  The stamps cost time themselves, so the sums are for shares, not for K1's time.
+enum : uint32_t {
+    K1P_CARRIES,     // carries from the bytes in front of the slab
+    K1P_TMA,         // wait for the tile's bytes
+    K1P_CLASSIFY,    // phase A: load + classify every block
+    K1P_PASS2,       // pass 2: escapes, quote parity
+    K1P_WAIT,        // output offsets and in-string state from the scan warp (bar_S, bar_Q)
+    K1P_B_CLASSIFY,  // phase B: the classes step_events reads
+    K1P_B_ESCAPES,   // phase B: escapes inside strings -> dropped bytes
+    K1P_EVENTS,      // step_events
+    K1P_AGG,         // the slab's counts
+    K1P_STORE,       // the SlabAgg store, slab count and last structural, bar_R
+    K1P_SECTIONS
+};
+#if defined(SJ_K1_PROBE) && defined(__CUDACC__)
+__device__ unsigned long long sj_k1_probe_cycles[K1P_SECTIONS];
+#endif
+#if defined(SJ_K1_PROBE) && defined(__CUDA_ARCH__)
+// (lane k keeps the sum of section k; parse mode only)
+#define K1_PROBE_START        \
+    uint32_t probe_acc = 0;   \
+    long long probe_t = clock64();
+#define K1_PROBE(sec)                                              \
+    do {                                                           \
+        if (PARSE) {                                               \
+            __syncwarp();                                          \
+            const long long t_ = clock64();                        \
+            if (lane == (sec)) probe_acc += (uint32_t)(t_ - probe_t); \
+            probe_t = t_;                                          \
+        }                                                          \
+    } while (0)
+#define K1_PROBE_FLUSH                                                                             \
+    do {                                                                                           \
+        if (PARSE && lane < K1P_SECTIONS) atomicAdd(&sj_k1_probe_cycles[lane], (unsigned long long)probe_acc); \
+    } while (0)
+#else
+#define K1_PROBE_START
+#define K1_PROBE(sec) \
+    do {              \
+    } while (0)
+#define K1_PROBE_FLUSH \
+    do {               \
+    } while (0)
+#endif
+
 struct Stage1Result {
     uint32_t n_idx;           // total structurals found
     uint32_t error;           // != 0: control character (< 0x20) inside a string
@@ -191,13 +238,15 @@ __device__ __forceinline__ SlowMasks classify_block_slow(const uint32_t (&w)[16]
 // bit streams), after which every class is a Boolean function of the planes evaluated for
 // 32 bytes per LOP3: no per-class compares, no flag gathering, and tab / LF / CR / control
 // masks come for free.  K1's class set differs from the streaming pass's (classify_planes2),
-// so the Boolean functions stay apart.  About 230 instructions per 64-byte block for
+// so the Boolean functions stay apart; the parse mode takes the two planes it needs on top of
+// them (parse_planes) from classify_planes2 on the same transpose.  About 230 instructions per 64-byte block for
 // all six masks, against 464 (4 masks) to 750 (with the control-character pass) for the
 // word-wise SWAR compares above; those stay as an independent second implementation that the
 // test hook sj_test_block_masks cross-checks against this one on every block.
 // ---------------------------------------------------------------------------------
 struct PlaneMasks {
     uint64_t bs, qt, st, ws, ct, nl;
+    uint64_t px, py;  // parse mode: X / Y of parse_planes (s2s_core.h)
 };
 
 struct HalfMasks {
@@ -234,7 +283,10 @@ __device__ __forceinline__ PlaneMasks classify_block_planes(const uint32_t (&w)[
     bit_planes32(&w[0], p0);
     bit_planes32(&w[8], p1);
     HalfMasks a = classify_planes(p0), b = classify_planes(p1);
+    const ParsePlanes pa = parse_planes(p0), pb = parse_planes(p1);
     PlaneMasks m;
+    m.px = mk64(pa.x, pb.x);
+    m.py = mk64(pa.y, pb.y);
     m.bs = mk64(a.bs, b.bs);
     m.qt = mk64(a.qt, b.qt);
     m.st = mk64(a.st, b.st);
@@ -696,8 +748,8 @@ __device__ __forceinline__ void load_block_words(const uint8_t* buf, uint32_t la
 
 // bytes at or beyond `len` read as 0x20 (find_structural_bits_amd64.s:134-155).
 // PARSE: the streaming parse's stage 1.  No index is extracted or written (out / out_cap are not used); phase B adds
-// up, per slab, the counts stage 2 needs (SlabAgg: the same step_events / agg_add_step the emulator's counting pass
-// runs) from the masks it has at hand, with the slab's bytes still in shared memory.
+// up, per slab, the counts stage 2 needs (SlabAgg: the same step_events / agg_lane_add / agg_warp_finish the emulator's
+// counting pass runs) from one classification per block, run behind bar_P, with the slab's bytes still in shared memory.
 template <bool NDJSON, bool DELTAS, bool PARSE = false>
 __global__ void __launch_bounds__(S1_THREADS, S1_CTAS_PER_SM) stage1_flatten_kernel(const Stage1Params p) {
     extern __shared__ __align__(128) uint8_t smem[];
@@ -851,6 +903,7 @@ __global__ void __launch_bounds__(S1_THREADS, S1_CTAS_PER_SM) stage1_flatten_ker
         return (t < p.ntiles && ss < p.len && ss > lane) ? (uint32_t)p.msg[ss - 1 - lane] : 0x20u;
     };
     uint32_t peekc = peek_load(tile);
+    K1_PROBE_START
 
     while (tile < p.ntiles || have_prev) {
         const bool cur = tile < p.ntiles;  // CTA-uniform
@@ -873,6 +926,7 @@ __global__ void __launch_bounds__(S1_THREADS, S1_CTAS_PER_SM) stage1_flatten_ker
             const uint32_t n = __ffs(~(peek_bs >> 1)) - 1;
             prevc_esc = n == 31 ? backslash_run_before(p.msg, slab_start - 1) & 1 : n & 1;
         }
+        K1_PROBE(K1P_CARRIES);
         if (cur) {
             mbar_wait(&bars[b], (phasebits >> b) & 1);
             phasebits ^= 1u << b;
@@ -885,17 +939,28 @@ __global__ void __launch_bounds__(S1_THREADS, S1_CTAS_PER_SM) stage1_flatten_ker
             for (uint32_t o = (uint32_t)(p.len - slab_start) + lane; o < S1_SLAB_BYTES; o += 32) wbuf[o] = 0x20;
             __syncwarp();
         }
+        K1_PROBE(K1P_TMA);
 
         // ---------------- phase A: classify, escape analysis, slab quote parity ----------------
         uint64_t qb[S1_STEPS], st[S1_STEPS], ws[S1_STEPS], ct[S1_STEPS], nl[S1_STEPS], bsm[S1_STEPS], qmr[S1_STEPS];
+        uint64_t px[S1_STEPS], py[S1_STEPS];  // PARSE: the rest of the classes phase B reads (parse_planes)
         uint32_t slab_par = 0;
         uint32_t cinbits = 0;  // PARSE: bit s = escape carry into the lane's block of step s
+        uint32_t ctbits = 0;   // PARSE: bit s / bit 8 + s = a control character inside / outside the slab-relative quote mask of step s
         uint32_t* const stage = reinterpret_cast<uint32_t*>(smem + (size_t)b * S1_TILE_BYTES + (size_t)warp * S1_SLAB_BYTES);
         const uint32_t pslab_pos = (uint32_t)(((uint64_t)prev_tile * S1_WARPS + warp) * S1_SLAB_BYTES);
 #pragma unroll
         for (int s = 0; s < S1_STEPS; s++) {
-            qb[s] = st[s] = ws[s] = ct[s] = nl[s] = bsm[s] = qmr[s] = 0;
-            if (active) {
+            qb[s] = st[s] = ws[s] = ct[s] = nl[s] = bsm[s] = qmr[s] = px[s] = py[s] = 0;
+            if (active && PARSE) {
+                // parse mode: the quote parity first, from the quotes and backslashes alone (the word-wise classifier),
+                // so that chain 1 starts early; the other classes come after bar_P, under the look-back
+                uint32_t w[16];
+                load_block_words(buf + s * S1_STEP_BYTES, lane, w);
+                const BlockMasks m = classify_block(w);
+                bsm[s] = rotl16x((uint32_t)m.bs, (uint32_t)(m.bs >> 32), rsel);
+                qb[s] = rotl16x((uint32_t)m.qt, (uint32_t)(m.qt >> 32), rsel);
+            } else if (active) {
                 uint32_t w[16];
                 load_block_words(buf + s * S1_STEP_BYTES, lane, w);
                 PlaneMasks m = classify_block_planes(w);
@@ -907,6 +972,7 @@ __global__ void __launch_bounds__(S1_THREADS, S1_CTAS_PER_SM) stage1_flatten_ker
                 if (NDJSON) nl[s] = rotl16x((uint32_t)m.nl, (uint32_t)(m.nl >> 32), rsel);
             }
         }
+        K1_PROBE(K1P_CLASSIFY);
         if (active) {
             // pass 2: everything that needs votes across the warp
 #pragma unroll
@@ -937,6 +1003,7 @@ __global__ void __launch_bounds__(S1_THREADS, S1_CTAS_PER_SM) stage1_flatten_ker
                 if (p.bsmap && lane == 0) p.bsmap[slab * S1_STEPS + s] = hasbs;
             }
         }
+        K1_PROBE(K1P_PASS2);
         // P: the slab's parity is written and the warp is done with buffer b^1.  When the last worker
         // has signalled, the scan warp issues the TMA of the next tile into b^1 and starts chain 1 of
         // this tile; nobody waits here, so the warps drift apart and the ALU-bound classification of
@@ -946,6 +1013,24 @@ __global__ void __launch_bounds__(S1_THREADS, S1_CTAS_PER_SM) stage1_flatten_ker
             mbar_arrive(bar_P);
         }
         const uint32_t peek_next = peek_load(tile + G);
+        if (PARSE && active) {
+            // the classes phase B reads, from one bit-sliced classification of each block (the slab's bytes stay in
+            // buffer b: parse mode stages nothing over them)
+#pragma unroll
+            for (int s = 0; s < S1_STEPS; s++) {
+                uint32_t w[16];
+                load_block_words(buf + s * S1_STEP_BYTES, lane, w);
+                const PlaneMasks m = classify_block_planes(w);
+                st[s] = rotl16x((uint32_t)m.st, (uint32_t)(m.st >> 32), rsel);
+                ws[s] = rotl16x((uint32_t)m.ws, (uint32_t)(m.ws >> 32), rsel);
+                if (NDJSON) nl[s] = rotl16x((uint32_t)m.nl, (uint32_t)(m.nl >> 32), rsel);
+                px[s] = rotl16x((uint32_t)m.px, (uint32_t)(m.px >> 32), rsel);
+                py[s] = rotl16x((uint32_t)m.py, (uint32_t)(m.py >> 32), rsel);
+                const uint64_t ctm = rotl16x((uint32_t)m.ct, (uint32_t)(m.ct >> 32), rsel);
+                ctbits |= ((ctm & qmr[s]) != 0 ? 1u : 0u) << s | ((ctm & ~qmr[s]) != 0 ? 1u : 0u) << (8 + s);
+            }
+            K1_PROBE(K1P_CLASSIFY);
+        }
         // ---------------- extraction of the previous tile's structurals ----------------
         // the positions are staged over the warp's own slab of this tile (dead: this warp alone read
         // it, in phase A above)
@@ -993,6 +1078,7 @@ __global__ void __launch_bounds__(S1_THREADS, S1_CTAS_PER_SM) stage1_flatten_ker
             // prevc not a quote: its quote_mask bit equals the in-string state after it (= par_in)
             pp_carry = is_q | is_ws | (is_st & (par_in ^ 1));
         }
+        K1_PROBE(K1P_WAIT);
 
         // ---------------- phase B: quote mask, finalize, counts ----------------
         uint32_t err = 0;
@@ -1004,33 +1090,26 @@ __global__ void __launch_bounds__(S1_THREADS, S1_CTAS_PER_SM) stage1_flatten_ker
             DevWarp wp;
             const GlobalReader g{p.msg, p.len};
             const SlabReader rd{buf, slab_start, active ? (uint32_t)min((uint64_t)S1_SLAB_BYTES, p.len - slab_start) : 0u, p.msg, p.len};
-            SlabAgg run = agg_zero();
-            uint32_t trail = 0, hasq = 0, s2err = 0, hd_drop = 0;
+            LaneAgg la = lane_agg_zero();
+            uint32_t s2err = 0, hd_drop = 0;
+            err = (par_in ? ctbits >> 8 : ctbits & 0xffu) != 0;  // find_quote_mask_and_bits_amd64.s:69-80
             uint32_t ppc = pp_carry;
             uint32_t recc = (NDJSON && active && !par_in && slab > 0) ? record_carry_in(wp, g, slab_start, peekc) : 0u;
+            K1_PROBE(K1P_CARRIES);
 #pragma unroll
             for (int s = 0; s < S1_STEPS; s++) {
                 const uint64_t qm = qmr[s] ^ flip;
-                if (ct[s] & qm) err = 1;  // find_quote_mask_and_bits_amd64.s:69-80
                 const uint64_t step_start = slab_start + (uint64_t)s * S1_STEP_BYTES;
                 uint64_t fin = 0;
                 if (active && step_start < p.len) {  // warp-uniform
-                    uint32_t w[16];
-                    load_block_words(buf + s * S1_STEP_BYTES, lane, w);
-                    const Class64 c = classify_block2(w);
-                    Class64 m;
-                    m.open = rotl16x((uint32_t)c.open, (uint32_t)(c.open >> 32), rsel);
-                    m.close = rotl16x((uint32_t)c.close, (uint32_t)(c.close >> 32), rsel);
-                    m.cc = rotl16x((uint32_t)c.cc, (uint32_t)(c.cc >> 32), rsel);
-                    m.numc = rotl16x((uint32_t)c.numc, (uint32_t)(c.numc >> 32), rsel);
-                    m.atomc = rotl16x((uint32_t)c.atomc, (uint32_t)(c.atomc >> 32), rsel);
+                    Class64 m = classes_from_parse_planes(st[s], px[s], py[s]);
                     m.ws = ws[s];
                     m.nl = nl[s];
+                    K1_PROBE(K1P_B_CLASSIFY);
                     // escapes inside strings -> the bytes they drop from Strings.B; what an escape that starts in front
                     // of the step leaves behind its start: head_info at the slab start, the previous step's last lane
                     // inside the slab
-                    const uint64_t bsr = rotl16x((uint32_t)c.bs, (uint32_t)(c.bs >> 32), rsel);
-                    const uint64_t Ein = escape_starts(bsr, (cinbits >> s) & 1u) & qm;
+                    const uint64_t Ein = escape_starts(bsm[s], (cinbits >> s) & 1u) & qm;
                     if (s == 0) {
                         const HeadInfo hd = head_info(wp, g, step_start, par_in != 0, peekc);
                         hd_drop = hd.drop;
@@ -1063,18 +1142,21 @@ __global__ void __launch_bounds__(S1_THREADS, S1_CTAS_PER_SM) stage1_flatten_ker
                     if (lane == 0) D |= hd_drop;
                     hd_drop = next_drop;
                     const uint64_t K = qm & ~qb[s] & ~D;
+                    K1_PROBE(K1P_B_ESCAPES);
                     const StepEvents e = step_events(wp, m, qm, qb[s], K, NDJSON ? 1u : 0u, ppc, recc);
-                    agg_add_step(wp, e, run, trail, hasq);
-                    run.last = agg_last_step(wp, e.S, run.last, [&](uint32_t o) { return (uint32_t)buf[s * S1_STEP_BYTES + o]; });
+                    K1_PROBE(K1P_EVENTS);
+                    agg_lane_add(la, e, s);
+                    K1_PROBE(K1P_AGG);
                     fin = e.S;
                 }
                 S_prev[s] = fin;
                 slab_count += __popcll(fin);
             }
             if (__any_sync(FULL, s2err) && lane == 0) atomicOr(p.s2_error, 1u);
-            if (active && lane == 0) {
-                run.trail = (hasq ? TRAIL_HASQ : 0u) | (trail & ~TRAIL_HASQ);
-                p.agg[slab] = run;
+            if (active) {  // warp-uniform
+                const SlabAgg run = agg_warp_finish(wp, la, S_prev, [&](uint32_t s, uint32_t o) { return (uint32_t)buf[s * S1_STEP_BYTES + o]; });
+                K1_PROBE(K1P_AGG);
+                if (lane == 0) p.agg[slab] = run;
             }
         } else {
 #pragma unroll
@@ -1117,6 +1199,7 @@ __global__ void __launch_bounds__(S1_THREADS, S1_CTAS_PER_SM) stage1_flatten_ker
         // R: slab counts of the tile are written (the same lane 0 wrote them)
         if (lane == 0) mbar_arrive(bar_R);
         itpar ^= 1;
+        K1_PROBE(K1P_STORE);
 
         have_prev = cur;
         prev_tile = tile;
@@ -1125,6 +1208,7 @@ __global__ void __launch_bounds__(S1_THREADS, S1_CTAS_PER_SM) stage1_flatten_ker
         tile += G;
         b ^= 1;
     }
+    K1_PROBE_FLUSH;
 }
 
 // After K1: rebase the first delta of every tile on the last structural of the tiles in
