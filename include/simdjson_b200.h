@@ -299,6 +299,11 @@ int sj_test_set_string_hash_bits(sj_ctx* ctx, int bits);
  * returns SJ_ERR_STAGE2).  A defect of the library, never a verdict on the input: tests expect 0 on every input.
  */
 int sj_test_stage2_internal(sj_ctx* ctx, uint32_t* word);
+/*
+ * sj_test_stage1_ctas: the CTAs of stage 1's cooperative grid on the context's device (one per SM).  Stage 1 deals its
+ * tiles round-robin over them, so tests place documents on the edge of a grid round with it.
+ */
+int sj_test_stage1_ctas(sj_ctx* ctx, uint32_t* ctas);
 
 /*
  * ParseNDStream (simdjson_amd64.go:116-215) inside the library: the caller pushes the bytes of an
