@@ -212,8 +212,9 @@ int sj_parse_count_where(sj_ctx* ctx, const uint8_t* msg, size_t len, uint32_t f
  * than 2^32 - 1 words returns SJ_ERR_TOO_LARGE.  *rows and *str_bytes are exact even on SJ_ERR_CAPACITY (rows > row_cap
  * or str_bytes > str_cap), when nothing is written; out may be NULL to ask for the sizes.
  * sj_find_device: message, tape, strings and out in device memory, with their lengths (every read stays inside them).
- * On the tape this context's last parse left in HBM the rows are stage 2's root list; on any other tape they are found
- * on the device: the 'r' words that point forward and are not the value word of a string or number (read from word 0),
+ * On the tape this context's last parse left in HBM the rows are stage 2's root list, until the next parse or an
+ * sj_deserialize_device that writes over any part of that tape (after either it is a foreign tape); on any other
+ * tape they are found on the device: the 'r' words that point forward and are not the value word of a string or number (read from word 0),
  * which on every tape the parser or sj_deserialize_device writes are the roots ForEach visits.  sj_parse_find: HOST message in, parse and find on the device, only the columns are copied to `out`
  * (host memory); parse errors return the parse codes.
  */

@@ -79,7 +79,10 @@ struct sj_ctx {
     // tape and the scan that finds it, and the output of an sj_parse_* call before its copy to the host
     DevBuf args, scratch, sz_tab, tc_roots, tc_scan, staging;
     uint32_t sz_hash_bits = 0;  // test hook: keep only this many bits of the dedup hash (0 = all)
-    // what the last successful stage 2 of this context left in device memory (valid until the next call)
+    // what the last successful stage 2 of this context left in device memory.  The next parse clears last_tape, and so
+    // does an sj_deserialize_device that writes over any part of that tape: tape_rows takes last_rootpos as the rows of
+    // a tape at last_tape of last_tape_len words only while it is set.  A caller's own writes to that buffer are not
+    // seen: the consumers take it as the tape the parse left there.
     const uint32_t* last_rootpos = nullptr;  // stage 2's root list (slot of every record's root-open word, [0] implicit)
     uint64_t last_records = 0;               // record boundaries = roots - 1
     const uint64_t* last_tape = nullptr;
