@@ -44,7 +44,8 @@ extern "C" {
 #define SJ_STREAM_BUSY 9  /* sj_stream_close_input: every slot is in use -- take a result first, then call again */
 #define SJ_ERR_EXCHANGE 10 /* sj_parse_nd_sharded_count: a peer's totals did not arrive within the exchange's time limit */
 #define SJ_ERR_PEER 11     /* sj_parse_nd_sharded_count: a peer's shard failed before its totals existed (the whole ParseND fails) */
-#define SJ_ERR_UNSUPPORTED 12 /* sj_deserialize_device: the stream has S2 or zstd blocks (read them on the CPU) */
+#define SJ_ERR_UNSUPPORTED 12 /* sj_deserialize_device: zstd blocks, or S2 blocks outside SJ_COMPRESS_FAST (read them on the CPU);
+                                 sj_ctx_set_compress_mode: a mode that needs zstd */
 /* negative values: -(1000 + cudaError_t) */
 
 #define SJ_MAX_MESSAGE 0x7fffff00ull /* positions are uint32, string lengths keep one flag bit */
@@ -282,7 +283,8 @@ int sj_parse_marshal(sj_ctx* ctx, const uint8_t* msg, size_t len, uint32_t flags
  * sj_deserialize_device: stream in device memory to tape, Strings.B and message in device memory.  Accepted exactly when
  * the reference's Deserialize on a zeroed tape returns no error and does not panic, every '{' / '[' names a later word
  * that holds its matching close, and no close is named twice; the output then equals the reference's.  Versions 0-3 are
- * read alike and bytes behind the values block are ignored.  S2 / zstd blocks return SJ_ERR_UNSUPPORTED, any other
+ * read alike and bytes behind the values block are ignored.  S2 / zstd blocks return SJ_ERR_UNSUPPORTED (S2 blocks are
+ * read in SJ_COMPRESS_FAST mode, below), any other
  * rejection SJ_ERR_ARGUMENT, over SJ_MAX_MARSHAL_TAPE tape words or tags SJ_ERR_TOO_LARGE.  The three sizes are exact on
  * SJ_ERR_CAPACITY; nothing is written unless the call succeeds.
  * sj_test_set_string_hash_bits: keep only `bits` bits of the dedup hash (0 = all), to force hash collisions in tests.
@@ -294,6 +296,33 @@ int sj_deserialize_device(sj_ctx* ctx, const uint8_t* d_in, size_t in_len, uint6
                           uint8_t* d_strings, size_t strings_cap, size_t* strings_len, uint8_t* d_msg, size_t msg_cap,
                           size_t* msg_len);
 int sj_test_set_string_hash_bits(sj_ctx* ctx, int bits);
+/*
+ * Serializer.CompressMode (parsed_serialize.go:93-115) of a context's Serializer calls.  SJ_COMPRESS_NONE (the default):
+ * the streams and the Deserialize verdicts above.  SJ_COMPRESS_FAST: sj_serialize_device / sj_parse_serialize write the
+ * message, tags and values blocks as block type 1, an S2 stream each (s2.cuh), and sj_deserialize_device reads S2 blocks
+ * too.  SJ_COMPRESS_DEFAULT and SJ_COMPRESS_BEST need zstd, which the device does not have: SJ_ERR_UNSUPPORTED, and the
+ * mode stays as it was; zstd blocks in a stream stay SJ_ERR_UNSUPPORTED in every mode.
+ * An S2 block written here: the stream identifier ff 06 00 00 "S2sTwO" (no bytes at all for an empty block), then one
+ * chunk per 64 KiB of input, compressed (0x00, literals and copies with 1- and 2-byte offsets only: the Snappy subset)
+ * or stored (0x01) when compressing would not make it shorter, each with the masked CRC-32C of its bytes.  The stream
+ * is deterministic: it depends only on the tape's content, as the uncompressed one does.
+ * An S2 block read here, after the header checks above, is accepted as s2.Reader fills the block's uncompressed size:
+ * the first chunk is an identifier ("S2sTwO", or "sNaPpY": then no chunk may decode to more than 64 KiB), which may
+ * repeat; 0x00 / 0x01 chunks are at least 4 bytes long, decode to at most 4 MiB, in full, to their stated length and CRC;
+ * 0x80 - 0xfe chunks are skipped, 0x02 - 0x7f rejected; blocks are S2 (copy offset 0 of a 1-byte-offset copy repeats
+ * the last offset).  Chunks are read until the size is filled and nothing behind that chunk is read; running out of
+ * chunks first is rejected; a block of size 0 reads nothing.  Every such rejection is SJ_ERR_ARGUMENT.  A stream is
+ * accepted exactly when it is accepted with each S2 block replaced by its inflated bytes as an uncompressed block.
+ * sj_test_s2_encode / sj_test_s2_decode: the codec alone on device buffers -- one S2 stream of `in` (identifier and
+ * chunks; *out_len exact on SJ_ERR_CAPACITY), and one S2 stream read as a block of `want` uncompressed bytes.
+ */
+#define SJ_COMPRESS_NONE 0
+#define SJ_COMPRESS_FAST 1
+#define SJ_COMPRESS_DEFAULT 2
+#define SJ_COMPRESS_BEST 3
+int sj_ctx_set_compress_mode(sj_ctx* ctx, int mode);
+int sj_test_s2_encode(sj_ctx* ctx, const uint8_t* d_in, size_t len, uint8_t* d_out, size_t cap, size_t* out_len);
+int sj_test_s2_decode(sj_ctx* ctx, const uint8_t* d_in, size_t len, uint8_t* d_out, size_t want, size_t* got);
 /*
  * sj_test_stage2_internal: the internal-error word of the last parse through the streaming stage 2 (copy_strings):
  * non-zero when the tape writer's counts of a slab differed from the ones stage 1 added up for it (the parse then

@@ -27,6 +27,7 @@
 #include "find.cuh"
 #include "marshal.cuh"
 #include "serialize.cuh"
+#include "s2.cuh"
 #include "gen.cuh"
 #include "exchange.cuh"
 
@@ -139,7 +140,7 @@ extern "C" const char* sj_error_string(int rc) {
     case SJ_STREAM_BUSY: return "every stream slot is in use";
     case SJ_ERR_EXCHANGE: return "sharded ParseND: a peer's totals did not arrive in time";
     case SJ_ERR_PEER: return "sharded ParseND: a peer's shard failed";
-    case SJ_ERR_UNSUPPORTED: return "serialized stream has S2 or zstd blocks: only uncompressed blocks are read on the device";
+    case SJ_ERR_UNSUPPORTED: return "serialized stream has zstd blocks, or S2 blocks outside CompressFast mode, or the compress mode needs zstd";
     default: return rc < 0 ? cudaGetErrorString((cudaError_t)(-rc - 1000)) : "unknown error";
     }
 }
@@ -212,7 +213,8 @@ extern "C" void sj_ctx_destroy(sj_ctx* c) {
     exchange_release(c);
     DevBuf* bufs[] = {&c->msg,     &c->idx,      &c->desc,     &c->result, &c->s2a,     &c->s2b,    &c->s2c,
                       &c->tape,    &c->strings,  &c->test_in,  &c->test_out, &c->test_aux, &c->args, &c->scratch,
-                      &c->sz_tab,  &c->tc_roots, &c->tc_scan,  &c->staging};
+                      &c->sz_tab,  &c->tc_roots, &c->tc_scan,  &c->staging, &c->s2_raw, &c->s2_slots, &c->s2_list,
+                      &c->s2_out};
     for (DevBuf* b : bufs) b->release();
     if (c->host_result) cudaFreeHost(c->host_result);
     free(c->pending);
@@ -568,6 +570,7 @@ extern "C" int sj_test_flatten_bits(sj_ctx* c, const uint64_t* masks, size_t nma
 #include "sj_consume.inl"
 #include "sj_marshal.inl"
 #include "sj_find.inl"
+#include "sj_s2.inl"
 #include "sj_serialize.inl"
 #include "sj_stream.inl"
 #include "sj_gen.inl"

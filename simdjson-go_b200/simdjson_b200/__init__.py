@@ -10,7 +10,8 @@ import ctypes as C
 import numpy as np
 
 from . import _lib
-from ._lib import (ERR_CAPACITY, ERR_STAGE1, ERR_STAGE2, ERR_UNSUPPORTED, FIND_CONVERT, FIND_CORRUPT, FIND_KIND_BOOL,
+from ._lib import (COMPRESS_BEST, COMPRESS_DEFAULT, COMPRESS_FAST, COMPRESS_NONE, ERR_CAPACITY, ERR_STAGE1, ERR_STAGE2,
+                   ERR_UNSUPPORTED, FIND_CONVERT, FIND_CORRUPT, FIND_KIND_BOOL,
                    FIND_KIND_ELEMENT, FIND_KIND_FLOAT64, FIND_KIND_INT64, FIND_KIND_STRING, FIND_KIND_UINT64,
                    FIND_NOT_FOUND, FIND_NOT_OBJECT, FIND_OK, FLAG_COPY_STRINGS, FLAG_NDJSON, OK, SjError, Stage1Info)
 
@@ -18,6 +19,9 @@ JSONVALUEMASK = 0xFF_FFFF_FFFF_FFFF  # parsed_json.go:26
 JSONTAGOFFSET = 56
 STRINGBUFBIT = 0x80_0000_0000_0000   # parsed_json.go:29
 M64 = (1 << 64) - 1
+
+# parsed_serialize.go:79-91 CompressMode.  Default and Best need zstd, which the device does not have.
+CompressNone, CompressFast, CompressDefault, CompressBest = COMPRESS_NONE, COMPRESS_FAST, COMPRESS_DEFAULT, COMPRESS_BEST
 
 
 def SupportedCPU():
@@ -45,6 +49,16 @@ class Context:
         if rc != OK:
             raise SjError(rc)
         self.h = h
+        self.compress_mode = CompressNone
+
+    def set_compress_mode(self, mode):
+        """Serializer.CompressMode of this context's serialize / deserialize calls: CompressNone (default, uncompressed
+        blocks) or CompressFast (S2 blocks, written and read); CompressDefault / CompressBest raise SjError
+        (SJ_ERR_UNSUPPORTED: they need zstd)"""
+        rc = self.L.sj_ctx_set_compress_mode(self.h, int(mode))
+        if rc != OK:
+            raise SjError(rc)
+        self.compress_mode = int(mode)
 
     def set_stage2_impl(self, impl):
         """0 = streaming stage-2 kernels whenever copy_strings is on (default), 1 = per-structural kernels always"""
@@ -269,6 +283,32 @@ class Context:
             return rc, sizes, None
         return rc, sizes, (tape[:sizes[0]], strings[:sizes[1]], message[:sizes[2]])
 
+    def s2_encode(self, data, out=None):
+        """test hook: one S2 stream (identifier and chunks) of `data` (uint8 tensor on this context's device), written by
+        the device encoder into `out` or a new tensor: (rc, length, the view holding it); SJ_ERR_CAPACITY when `out` is
+        too small (the length is still exact)"""
+        import torch
+        ip, il = _ptr_len(data)
+        n = C.c_size_t(0)
+        if out is None:
+            rc = self.L.sj_test_s2_encode(self.h, ip, il, None, 0, C.byref(n))
+            if rc not in (OK, ERR_CAPACITY):
+                return rc, n.value, None
+            out = torch.empty(max(n.value, 1), dtype=torch.uint8, device=data.device)
+        rc = self.L.sj_test_s2_encode(self.h, ip, il, out.data_ptr(), out.numel(), C.byref(n))
+        return rc, n.value, out[:n.value]
+
+    def s2_decode(self, stream, want, out=None):
+        """test hook: the S2 stream `stream` (uint8 tensor) read as a block of `want` uncompressed bytes by the device
+        decoder, into `out` or a new tensor: (rc, the view of its `want` bytes or None)"""
+        import torch
+        ip, il = _ptr_len(stream)
+        if out is None:
+            out = torch.empty(max(want, 1), dtype=torch.uint8, device=stream.device)
+        got = C.c_size_t(0)
+        rc = self.L.sj_test_s2_decode(self.h, ip, il, out.data_ptr(), want, C.byref(got))
+        return rc, (out[:got.value] if rc == OK else None)
+
     def set_string_hash_bits(self, bits):
         """test hook: keep only `bits` bits of the serializer's string hash (0 = all), to force collisions"""
         rc = self.L.sj_test_set_string_hash_bits(self.h, int(bits))
@@ -474,17 +514,39 @@ def ParseND(b, reuse=None, copy_strings=True, ctx=None):
 
 
 class Serializer:
-    """parsed_serialize.go:44 Serializer, on the default context's device.  Blocks are always uncompressed
-    (CompressNone), and strings are deduplicated exactly (first occurrence), so the stream does not depend on
-    copy_strings; the reference's Deserialize reads it."""
+    """parsed_serialize.go:44 Serializer, on the default context's device.  Blocks are uncompressed (CompressNone) unless
+    CompressMode(CompressFast) asks for S2 blocks, and strings are deduplicated exactly (first occurrence), so the stream
+    does not depend on copy_strings; the reference's Deserialize reads it."""
 
     def __init__(self, ctx=None):
         self.ctx = ctx
+        self.mode = CompressNone
+
+    def CompressMode(self, c):
+        """parsed_serialize.go:93 CompressMode: CompressNone or CompressFast; CompressDefault / CompressBest raise
+        SjError (SJ_ERR_UNSUPPORTED: zstd)"""
+        if c in (CompressDefault, CompressBest):
+            raise SjError(ERR_UNSUPPORTED)
+        if c not in (CompressNone, CompressFast):
+            raise ValueError("unknown compression mode")
+        self.mode = c
+
+    def _call(self, fn):
+        """fn(ctx) with the context in this Serializer's compress mode, restored afterwards"""
+        ctx = self.ctx or default_context()
+        before = ctx.compress_mode
+        ctx.set_compress_mode(self.mode)
+        try:
+            return fn(ctx)
+        finally:
+            ctx.set_compress_mode(before)
 
     def Serialize(self, pj):
         """the v3 stream of pj (a ParsedJson) as bytes"""
+        return self._call(lambda ctx: self._serialize(ctx, pj))
+
+    def _serialize(self, ctx, pj):
         import torch
-        ctx = self.ctx or default_context()
         tape = torch.from_numpy(np.ascontiguousarray(pj.Tape, dtype=np.uint64).view(np.int64)).cuda()
         strs = torch.from_numpy(np.frombuffer(bytes(pj.Strings), dtype=np.uint8).copy()).cuda()
         msg = torch.from_numpy(np.frombuffer(bytes(pj.Message), dtype=np.uint8).copy()).cuda()
@@ -494,9 +556,12 @@ class Serializer:
         return out.cpu().numpy().tobytes()
 
     def Deserialize(self, src):
-        """a ParsedJson from a v3 stream with uncompressed blocks (SJ_ERR_UNSUPPORTED for S2 / zstd blocks)"""
+        """a ParsedJson from a v3 stream with uncompressed blocks, or S2 blocks in CompressFast mode (SJ_ERR_UNSUPPORTED for
+        zstd blocks, and for S2 blocks in CompressNone mode)"""
+        return self._call(lambda ctx: self._deserialize(ctx, src))
+
+    def _deserialize(self, ctx, src):
         import torch
-        ctx = self.ctx or default_context()
         d = torch.from_numpy(np.frombuffer(bytes(src), dtype=np.uint8).copy()).cuda()
         rc, sizes, bufs = ctx.deserialize_device(d)
         if rc != OK:

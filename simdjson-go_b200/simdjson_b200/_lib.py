@@ -22,13 +22,15 @@ EXPORTS = [
     "sj_stage1_launch", "sj_ctx_sync", "sj_event_record", "sj_event_elapsed_ms", "sj_kernel_launches",
     "sj_test_block_masks", "sj_test_geometry", "sj_test_finalize", "sj_test_flatten_bits", "sj_test_parse_strings",
     "sj_test_parse_numbers", "sj_count_where_device", "sj_parse_count_where", "sj_find_device", "sj_parse_find", "sj_marshal_device", "sj_parse_marshal", "sj_serialize_device", "sj_parse_serialize",
-    "sj_deserialize_device", "sj_test_set_string_hash_bits", "sj_test_stage2_internal", "sj_test_stage1_ctas", "sj_stream_create", "sj_stream_destroy",
+    "sj_deserialize_device", "sj_test_set_string_hash_bits", "sj_ctx_set_compress_mode", "sj_test_s2_encode", "sj_test_s2_decode", "sj_test_stage2_internal", "sj_test_stage1_ctas", "sj_stream_create", "sj_stream_destroy",
     "sj_stream_write", "sj_stream_close_input", "sj_stream_next", "sj_stream_release",
 ]
 STREAM_END, STREAM_EMPTY, STREAM_BUSY = 7, 8, 9
 # sj_find_device / sj_parse_find: cell statuses and path kinds
 FIND_OK, FIND_NOT_FOUND, FIND_NOT_OBJECT, FIND_CONVERT, FIND_CORRUPT = range(5)
 FIND_KIND_ELEMENT, FIND_KIND_INT64, FIND_KIND_UINT64, FIND_KIND_FLOAT64, FIND_KIND_BOOL, FIND_KIND_STRING = range(6)
+# Serializer.CompressMode (sj_ctx_set_compress_mode)
+COMPRESS_NONE, COMPRESS_FAST, COMPRESS_DEFAULT, COMPRESS_BEST = range(4)
 FIND_MAX_PATHS, FIND_MAX_SEGMENTS, FIND_MAX_SEGMENT_BYTES = 64, 32, 16384
 
 
@@ -163,6 +165,12 @@ def load():
     L.sj_deserialize_device.argtypes = [vp, vp, sz, vp, sz, szp, vp, sz, szp, vp, sz, szp]
     L.sj_test_set_string_hash_bits.restype = i32
     L.sj_test_set_string_hash_bits.argtypes = [vp, i32]
+    L.sj_ctx_set_compress_mode.restype = i32
+    L.sj_ctx_set_compress_mode.argtypes = [vp, i32]
+    L.sj_test_s2_encode.restype = i32
+    L.sj_test_s2_encode.argtypes = [vp, vp, sz, vp, sz, szp]
+    L.sj_test_s2_decode.restype = i32
+    L.sj_test_s2_decode.argtypes = [vp, vp, sz, vp, sz, szp]
     L.sj_test_stage2_internal.restype = i32
     L.sj_test_stage2_internal.argtypes = [vp, C.POINTER(u32)]
     L.sj_test_stage1_ctas.restype = i32

@@ -79,6 +79,14 @@ for tape in (own, own.clone()):
     rc, sizes, (t2, s2, m2) = ctx.deserialize_device(stream)
     assert rc == 0 and ctx.marshal_device(t2[:sizes[0]], s2[:sizes[1]], m2[:sizes[2]])[2].cpu().numpy().tobytes() == want_text
     n += 1
+# the S2 blocks of CompressFast (s2.cuh): KC1 / KC2 and KX1 / KX2 around the same calls
+from tests import s2_oracle
+ctx.set_compress_mode(1)
+rc, _, stream = ctx.serialize_device(own, strs, msg)
+assert rc == 0 and s2_oracle.inflate(stream.cpu().numpy().tobytes()) == want_stream
+rc, sizes, (t2, s2, m2) = ctx.deserialize_device(stream)
+assert rc == 0 and ctx.marshal_device(t2[:sizes[0]], s2[:sizes[1]], m2[:sizes[2]])[2].cpu().numpy().tobytes() == want_text
+ctx.set_compress_mode(0)
 # carries across slab / tile edges, long strings (warp-cooperative paths), dense brackets, number-heavy
 g = (__import__("ctypes").c_uint32 * 4)()
 ctx.L.sj_test_geometry(g)
