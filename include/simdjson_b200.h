@@ -44,8 +44,8 @@ extern "C" {
 #define SJ_STREAM_BUSY 9  /* sj_stream_close_input: every slot is in use -- take a result first, then call again */
 #define SJ_ERR_EXCHANGE 10 /* sj_parse_nd_sharded_count: a peer's totals did not arrive within the exchange's time limit */
 #define SJ_ERR_PEER 11     /* sj_parse_nd_sharded_count: a peer's shard failed before its totals existed (the whole ParseND fails) */
-#define SJ_ERR_UNSUPPORTED 12 /* sj_deserialize_device: zstd blocks, or S2 blocks outside SJ_COMPRESS_FAST (read them on the CPU);
-                                 sj_ctx_set_compress_mode: a mode that needs zstd */
+#define SJ_ERR_UNSUPPORTED 12 /* sj_deserialize_device: S2 blocks in SJ_COMPRESS_NONE mode, zstd blocks in SJ_COMPRESS_NONE /
+                                 SJ_COMPRESS_FAST mode (set SJ_COMPRESS_DEFAULT or SJ_COMPRESS_BEST to read them) */
 /* negative values: -(1000 + cudaError_t) */
 
 #define SJ_MAX_MESSAGE 0x7fffff00ull /* positions are uint32, string lengths keep one flag bit */
@@ -283,8 +283,8 @@ int sj_parse_marshal(sj_ctx* ctx, const uint8_t* msg, size_t len, uint32_t flags
  * sj_deserialize_device: stream in device memory to tape, Strings.B and message in device memory.  Accepted exactly when
  * the reference's Deserialize on a zeroed tape returns no error and does not panic, every '{' / '[' names a later word
  * that holds its matching close, and no close is named twice; the output then equals the reference's.  Versions 0-3 are
- * read alike and bytes behind the values block are ignored.  S2 / zstd blocks return SJ_ERR_UNSUPPORTED (S2 blocks are
- * read in SJ_COMPRESS_FAST mode, below), any other
+ * read alike and bytes behind the values block are ignored.  S2 / zstd blocks return SJ_ERR_UNSUPPORTED (they are
+ * read in the compressed modes, below), any other
  * rejection SJ_ERR_ARGUMENT, over SJ_MAX_MARSHAL_TAPE tape words or tags SJ_ERR_TOO_LARGE.  The three sizes are exact on
  * SJ_ERR_CAPACITY; nothing is written unless the call succeeds.
  * sj_test_set_string_hash_bits: keep only `bits` bits of the dedup hash (0 = all), to force hash collisions in tests.
@@ -300,8 +300,9 @@ int sj_test_set_string_hash_bits(sj_ctx* ctx, int bits);
  * Serializer.CompressMode (parsed_serialize.go:93-115) of a context's Serializer calls.  SJ_COMPRESS_NONE (the default):
  * the streams and the Deserialize verdicts above.  SJ_COMPRESS_FAST: sj_serialize_device / sj_parse_serialize write the
  * message, tags and values blocks as block type 1, an S2 stream each (s2.cuh), and sj_deserialize_device reads S2 blocks
- * too.  SJ_COMPRESS_DEFAULT and SJ_COMPRESS_BEST need zstd, which the device does not have: SJ_ERR_UNSUPPORTED, and the
- * mode stays as it was; zstd blocks in a stream stay SJ_ERR_UNSUPPORTED in every mode.
+ * too; zstd blocks stay SJ_ERR_UNSUPPORTED in SJ_COMPRESS_NONE and SJ_COMPRESS_FAST mode.  SJ_COMPRESS_DEFAULT: the
+ * tags block is written as block type 2, a zstd frame (zstd.cuh), the message and values blocks as S2; SJ_COMPRESS_BEST:
+ * all three as zstd.  Both read uncompressed, S2 and zstd blocks.  Any other mode is SJ_ERR_ARGUMENT.
  * An S2 block written here: the stream identifier ff 06 00 00 "S2sTwO" (no bytes at all for an empty block), then one
  * chunk per 64 KiB of input, compressed (0x00, literals and copies with 1- and 2-byte offsets only: the Snappy subset)
  * or stored (0x01) when compressing would not make it shorter, each with the masked CRC-32C of its bytes.  The stream
@@ -315,6 +316,37 @@ int sj_test_set_string_hash_bits(sj_ctx* ctx, int bits);
  * accepted exactly when it is accepted with each S2 block replaced by its inflated bytes as an uncompressed block.
  * sj_test_s2_encode / sj_test_s2_decode: the codec alone on device buffers -- one S2 stream of `in` (identifier and
  * chunks; *out_len exact on SJ_ERR_CAPACITY), and one S2 stream read as a block of `want` uncompressed bytes.
+ * A zstd block written here: nothing for an empty block (as the S2 path writes nothing: both read back as empty), else
+ * one frame -- single segment, Frame_Content_Size present, no checksum, no dictionary -- of one block per 64 KiB of
+ * input, the last flagged: a compressed block (raw literals, sequences with the predefined LL / OF / ML tables and new
+ * offsets only, matches inside the block) or a raw block when compressing would not make it shorter.  Deterministic.
+ * A zstd block read here (RFC 8878; the reference's decoder.DecodeAll and then the size check) is accepted when:
+ *  - frames: zero or more back to back fill the block exactly, each a zstd frame (magic 28 b5 2f fd) or a skippable
+ *    frame (magic 0x184D2A50 - 0x184D2A5F, skipped); all frames together decode to the block's uncompressed size;
+ *  - frame header: reserved bit 0; dictionary ID absent or 0; Frame_Content_Size, when present, equals the frame's
+ *    output; the window is the descriptor's, or the content size of a single-segment frame; with the checksum flag,
+ *    the low 32 bits of XXH64 (seed 0) of the frame's output match;
+ *  - blocks: raw, RLE and compressed (reserved type 3 rejected); a compressed block's content and decoded size at
+ *    most min(window, 128 KiB); raw and RLE blocks are not limited (see below); the last-block flag ends the frame;
+ *  - literals: raw, RLE, Huffman and treeless (the last Huffman table of the same frame, none: rejected), one stream or
+ *    four with the jump table; weights FSE-compressed or in the direct 4-bit form, at most 11 bits, completing a tree;
+ *  - sequences: every count encoding; predefined, RLE, FSE and repeat modes (repeat: a table of an earlier block of
+ *    the same frame); FSE descriptions whose counts add up exactly; literal lengths within the literals; every
+ *    bitstream (Huffman streams, FSE weights aside, and the sequences) ending exactly at its padding; a block with no
+ *    sequences ends behind its count byte;
+ *  - offsets: repeat offsets start at 1, 4, 8 in each frame; with literal length 0 a repeat code shifts by one (1 is
+ *    rep2, 2 rep3, 3 rep1 - 1, rejected when that is 0, as libzstd rejects it); a match reaching in front of the frame's
+ *    first byte is rejected (no dictionary).
+ * These rules are RFC 8878's and were checked against libzstd (through pyarrow) only; where the reference's Go decoder
+ * may differ from it -- the windows it refuses, an offset beyond the window inside the frame, a literal count below 6
+ * with four streams, FSE weights over 255 symbols -- this follows the RFC.  Two rules follow libzstd instead of the
+ * RFC: raw and RLE blocks larger than min(window, 128 KiB) are accepted (RFC 8878 3.1.1.2.2 limits every block type;
+ * libzstd limits compressed blocks only), and rep1 - 1 = 0 is rejected.  Every rejection is SJ_ERR_ARGUMENT; a stream
+ * whose zstd blocks end more than 4 GiB into the inflated stream returns SJ_ERR_TOO_LARGE (the decoder's per-byte
+ * sources are 32-bit positions).  A stream is accepted exactly when
+ * it is accepted with each compressed block replaced by its inflated bytes as an uncompressed block.
+ * sj_test_zstd_encode / sj_test_zstd_decode: the zstd codec alone, shaped like the S2 hooks: one frame of `in`, and
+ * zstd frames read as a block of `want` uncompressed bytes.
  */
 #define SJ_COMPRESS_NONE 0
 #define SJ_COMPRESS_FAST 1
@@ -323,6 +355,8 @@ int sj_test_set_string_hash_bits(sj_ctx* ctx, int bits);
 int sj_ctx_set_compress_mode(sj_ctx* ctx, int mode);
 int sj_test_s2_encode(sj_ctx* ctx, const uint8_t* d_in, size_t len, uint8_t* d_out, size_t cap, size_t* out_len);
 int sj_test_s2_decode(sj_ctx* ctx, const uint8_t* d_in, size_t len, uint8_t* d_out, size_t want, size_t* got);
+int sj_test_zstd_encode(sj_ctx* ctx, const uint8_t* d_in, size_t len, uint8_t* d_out, size_t cap, size_t* out_len);
+int sj_test_zstd_decode(sj_ctx* ctx, const uint8_t* d_in, size_t len, uint8_t* d_out, size_t want, size_t* got);
 /*
  * sj_test_stage2_internal: the internal-error word of the last parse through the streaming stage 2 (copy_strings):
  * non-zero when the tape writer's counts of a slab differed from the ones stage 1 added up for it (the parse then

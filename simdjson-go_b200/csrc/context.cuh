@@ -79,10 +79,11 @@ struct sj_ctx {
     // tape and the scan that finds it, and the output of an sj_parse_* call before its copy to the host
     DevBuf args, scratch, sz_tab, tc_roots, tc_scan, staging;
     uint32_t sz_hash_bits = 0;  // test hook: keep only this many bits of the dedup hash (0 = all)
-    // the Serializer's compress mode (SJ_COMPRESS_NONE / SJ_COMPRESS_FAST) and, within one call, the S2 codec's buffers
-    // (s2.cuh): the uncompressed stream and the encoder's chunk slots; the chunk list and the inflated blocks
+    // the Serializer's compress mode (SJ_COMPRESS_*) and, within one call, the S2 and zstd codecs' buffers (s2.cuh,
+    // zstd.cuh): the uncompressed stream and the encoders' chunk slots; the chunk, frame and block lists and the
+    // inflated blocks; the zstd encoder's sequences, and the decoder's literals, sequences and per-byte sources
     int compress_mode = 0;
-    DevBuf s2_raw, s2_slots, s2_list, s2_out;
+    DevBuf s2_raw, s2_slots, s2_list, s2_out, zx_seq, zx_src;
     // what the last successful stage 2 of this context left in device memory.  The next parse clears last_tape, and so
     // does an sj_deserialize_device that writes over any part of that tape: tape_rows takes last_rootpos as the rows of
     // a tape at last_tape of last_tape_len words only while it is set.  A caller's own writes to that buffer are not

@@ -10,8 +10,8 @@
 //                   the Snappy subset (literals, copies with 1- and 2-byte offsets); stored when that is not shorter.
 //                   The framed chunk goes into its own slot, its size into size[].
 //   KC2 sx_gather   the slots laid end to end behind the block heads.
-//   KX1 sx_list     one thread per S2 block walks its chunk headers, applies the framing rules (s2.Reader's chunk loop)
-//                   and lists the chunks that fill the block, with their output offsets.
+//   KX1 zx_list     (zstd.cuh) one thread per S2 block walks its chunk headers (sx_walk), applies the framing rules
+//                   (s2.Reader's chunk loop) and lists the chunks that fill the block, with their output offsets.
 //   KX2 sx_decode   one warp per listed chunk: literals and copies straight into global memory (a copy may reach back
 //                   4 MiB), the decoded length and the CRC checked.
 #pragma once
@@ -88,6 +88,7 @@ struct SxEncParams {
     const uint8_t* src[3];  // up to three inputs, each cut into chunks of S2_CHUNK bytes
     uint64_t len[3];
     uint32_t first[4];      // input b has chunks first[b] .. first[b + 1] - 1
+    uint32_t codec[3];      // input b's block type: 1 (S2, KC1's chunks) or 2 (zstd, KZ1's: zstd.cuh)
     uint32_t nchunks;
     uint8_t* slots;         // S2_SLOT bytes per chunk
     uint32_t* size;         // framed bytes of each chunk
@@ -146,21 +147,17 @@ __device__ __forceinline__ bool sx_emit_copy(uint8_t* out, uint32_t& o, uint32_t
     return true;
 }
 
-// The block of in[0, n) into out, by the whole warp: its length, or ~0u when it would not be shorter than n.  Steps of
-// 32 positions: every position hashes its 4 bytes, its candidate is the last earlier position of the step with the same
-// 4 bytes, else the table's (checked); then the table takes the step's positions (the last of each hash), and the
-// matches are taken greedily in position order, each extended 32 bytes at a time.  The next step starts behind the
-// step or behind the last match, whichever is later.
-__device__ uint32_t sx_compress_warp(const uint8_t* in, uint32_t n, uint8_t* out, uint16_t* tab) {
+// The match finder of KC1 (and of the zstd encoder, zstd.cuh) over in[0, n), by the whole warp: e.literal(s, L) and
+// e.copy(offset, L) in position order, false as soon as one of them is.  Steps of 32 positions: every position hashes
+// its 4 bytes, its candidate is the last earlier position of the step with the same 4 bytes, else the table's
+// (checked); then the table takes the step's positions (the last of each hash), and the matches are taken greedily in
+// position order, each extended 32 bytes at a time.  The next step starts behind the step or behind the last match,
+// whichever is later.  Matches are at least 4 bytes, offsets below n <= 65536.
+template <class Emit>
+__device__ bool sx_match_warp(const uint8_t* in, uint32_t n, uint16_t* tab, Emit& e) {
     const uint32_t lane = threadIdx.x & 31;
     for (uint32_t i = lane; i < (1u << S2_HASH_BITS) / 2; i += 32) reinterpret_cast<uint32_t*>(tab)[i] = 0xffffffffu;
     __syncwarp();
-    uint32_t o = 0;
-    for (uint32_t x = n; ; x >>= 7) {  // uvarint(n)
-        if (lane == 0) out[o] = (uint8_t)(x >= 0x80 ? (x | 0x80) : x);
-        o++;
-        if (x < 0x80) break;
-    }
     uint32_t emit = 0;
     for (uint32_t s = 0; n >= 4 && s <= n - 4;) {
         const uint32_t pos = s + lane;
@@ -198,14 +195,34 @@ __device__ uint32_t sx_compress_warp(const uint8_t* in, uint32_t n, uint8_t* out
                 }
                 len += 32;
             }
-            if (!sx_emit_literal(out, o, n, in + emit, p0 - emit) || !sx_emit_copy(out, o, n, p0 - c0, len)) return ~0u;
+            if (!e.literal(in + emit, p0 - emit) || !e.copy(p0 - c0, len)) return false;
             emit = p0 + len;
             m &= emit - s >= 32 ? 0u : ~((1u << (emit - s)) - 1);
         }
         s = max(s + 32, emit);
     }
-    if (!sx_emit_literal(out, o, n, in + emit, n - emit)) return ~0u;
-    return o;
+    return e.literal(in + emit, n - emit);
+}
+
+// sx_match_warp's elements as Snappy literals and copies at out + o, none ending past `limit`
+struct SxSnappyEmit {
+    uint8_t* out;
+    uint32_t o, limit;
+    __device__ bool literal(const uint8_t* s, uint32_t L) { return sx_emit_literal(out, o, limit, s, L); }
+    __device__ bool copy(uint32_t off, uint32_t L) { return sx_emit_copy(out, o, limit, off, L); }
+};
+
+// The block of in[0, n) into out, by the whole warp: its length, or ~0u when it would not be shorter than n
+__device__ uint32_t sx_compress_warp(const uint8_t* in, uint32_t n, uint8_t* out, uint16_t* tab) {
+    const uint32_t lane = threadIdx.x & 31;
+    uint32_t o = 0;
+    for (uint32_t x = n; ; x >>= 7) {  // uvarint(n)
+        if (lane == 0) out[o] = (uint8_t)(x >= 0x80 ? (x | 0x80) : x);
+        o++;
+        if (x < 0x80) break;
+    }
+    SxSnappyEmit e{out, o, n};
+    return sx_match_warp(in, n, tab, e) ? e.o : ~0u;
 }
 
 // KC1: chunk ci of its input, framed, into slot ci
@@ -221,6 +238,7 @@ __global__ void __launch_bounds__(S2_WARPS * 32) sx_encode_kernel(const SxEncPar
     if (ci >= p.nchunks) return;
     int b = 0;
     while (ci >= p.first[b + 1]) b++;
+    if (p.codec[b] != 1) return;
     const uint64_t at = (uint64_t)(ci - p.first[b]) * S2_CHUNK;
     const uint32_t n = (uint32_t)min((uint64_t)S2_CHUNK, p.len[b] - at);
     const uint8_t* in = p.src[b] + at;
@@ -340,26 +358,6 @@ __device__ bool sx_walk(const uint8_t* s, const SxBlock& blk, uint32_t i, SxChun
     }
     back->total[i] = filled;
     return true;
-}
-
-// KX1: the blocks (from the header, or the one block `one`), then one thread per S2 block
-__global__ void sx_list_kernel(const uint8_t* s, uint64_t len, SxBlock one, bool from_header, SxChunk* list, uint32_t cap,
-                               SxBack* back) {
-    __shared__ SxBlock b[4];
-    if (threadIdx.x == 0) {
-        if (from_header) {
-            sx_header_blocks(s, len, b);
-        } else {
-            b[0] = one;
-            for (int i = 1; i < 4; i++) b[i] = SxBlock{0, 0, 0, S2_NONE, 0};
-        }
-    }
-    __syncthreads();
-    const uint32_t i = threadIdx.x;
-    if (i >= 4) return;
-    back->type[i] = b[i].type;
-    back->total[i] = 0;
-    if (b[i].type == 1 && !sx_walk(s, b[i], i, list, cap, back)) atomicOr(&back->bad, 1u);
 }
 
 // a copy of L bytes from `off` back, by the whole warp: 32 bytes a step when off >= 32 (each step reads only bytes

@@ -27,7 +27,7 @@
 #include "find.cuh"
 #include "marshal.cuh"
 #include "serialize.cuh"
-#include "s2.cuh"
+#include "zstd.cuh"
 #include "gen.cuh"
 #include "exchange.cuh"
 
@@ -140,7 +140,7 @@ extern "C" const char* sj_error_string(int rc) {
     case SJ_STREAM_BUSY: return "every stream slot is in use";
     case SJ_ERR_EXCHANGE: return "sharded ParseND: a peer's totals did not arrive in time";
     case SJ_ERR_PEER: return "sharded ParseND: a peer's shard failed";
-    case SJ_ERR_UNSUPPORTED: return "serialized stream has zstd blocks, or S2 blocks outside CompressFast mode, or the compress mode needs zstd";
+    case SJ_ERR_UNSUPPORTED: return "serialized stream has S2 blocks in CompressNone mode, or zstd blocks in CompressNone / CompressFast mode";
     default: return rc < 0 ? cudaGetErrorString((cudaError_t)(-rc - 1000)) : "unknown error";
     }
 }
@@ -214,7 +214,7 @@ extern "C" void sj_ctx_destroy(sj_ctx* c) {
     DevBuf* bufs[] = {&c->msg,     &c->idx,      &c->desc,     &c->result, &c->s2a,     &c->s2b,    &c->s2c,
                       &c->tape,    &c->strings,  &c->test_in,  &c->test_out, &c->test_aux, &c->args, &c->scratch,
                       &c->sz_tab,  &c->tc_roots, &c->tc_scan,  &c->staging, &c->s2_raw, &c->s2_slots, &c->s2_list,
-                      &c->s2_out};
+                      &c->s2_out,  &c->zx_seq,   &c->zx_src};
     for (DevBuf* b : bufs) b->release();
     if (c->host_result) cudaFreeHost(c->host_result);
     free(c->pending);
@@ -571,6 +571,7 @@ extern "C" int sj_test_flatten_bits(sj_ctx* c, const uint64_t* masks, size_t nma
 #include "sj_marshal.inl"
 #include "sj_find.inl"
 #include "sj_s2.inl"
+#include "sj_zstd.inl"
 #include "sj_serialize.inl"
 #include "sj_stream.inl"
 #include "sj_gen.inl"

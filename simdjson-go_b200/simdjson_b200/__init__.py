@@ -20,7 +20,8 @@ JSONTAGOFFSET = 56
 STRINGBUFBIT = 0x80_0000_0000_0000   # parsed_json.go:29
 M64 = (1 << 64) - 1
 
-# parsed_serialize.go:79-91 CompressMode.  Default and Best need zstd, which the device does not have.
+# parsed_serialize.go:79-91 CompressMode.  Fast writes S2 blocks; Default zstd tags and S2 message and values; Best zstd
+# blocks throughout.
 CompressNone, CompressFast, CompressDefault, CompressBest = COMPRESS_NONE, COMPRESS_FAST, COMPRESS_DEFAULT, COMPRESS_BEST
 
 
@@ -53,8 +54,9 @@ class Context:
 
     def set_compress_mode(self, mode):
         """Serializer.CompressMode of this context's serialize / deserialize calls: CompressNone (default, uncompressed
-        blocks) or CompressFast (S2 blocks, written and read); CompressDefault / CompressBest raise SjError
-        (SJ_ERR_UNSUPPORTED: they need zstd)"""
+        blocks), CompressFast (S2 blocks), CompressDefault (zstd tags, S2 message and values) or CompressBest (zstd
+        blocks).  Deserialize reads S2 blocks in every mode but CompressNone, and zstd blocks in CompressDefault /
+        CompressBest only (SJ_ERR_UNSUPPORTED in the others)."""
         rc = self.L.sj_ctx_set_compress_mode(self.h, int(mode))
         if rc != OK:
             raise SjError(rc)
@@ -259,8 +261,9 @@ class Context:
         """Serializer.Deserialize (parsed_serialize.go:466) of a stream (uint8 tensor) on this context's device.  Writes
         into `tape` (int64 tensor), `strings` and `message` (uint8 tensors), or new tensors when all three are None.
         Returns (rc, (tape words, strings bytes, message bytes), (tape, strings, message) views).  rc is SJ_ERR_CAPACITY
-        when a buffer is too small (the sizes are still exact), SJ_ERR_UNSUPPORTED for S2 / zstd blocks and
-        SJ_ERR_ARGUMENT for a stream the device does not accept."""
+        when a buffer is too small (the sizes are still exact), SJ_ERR_UNSUPPORTED for S2 blocks in CompressNone mode
+        and zstd blocks in CompressNone / CompressFast mode, and SJ_ERR_ARGUMENT for a stream the device does not
+        accept."""
         import torch
         ip, il = _ptr_len(stream)
         tl, sl, ml = C.c_size_t(0), C.c_size_t(0), C.c_size_t(0)
@@ -307,6 +310,32 @@ class Context:
             out = torch.empty(max(want, 1), dtype=torch.uint8, device=stream.device)
         got = C.c_size_t(0)
         rc = self.L.sj_test_s2_decode(self.h, ip, il, out.data_ptr(), want, C.byref(got))
+        return rc, (out[:got.value] if rc == OK else None)
+
+    def zstd_encode(self, data, out=None):
+        """test hook: one zstd frame (single segment, content size, no checksum; nothing for empty data) of `data` (uint8
+        tensor on this context's device), written by the device encoder into `out` or a new tensor: (rc, length, the
+        view holding it); SJ_ERR_CAPACITY when `out` is too small (the length is still exact)"""
+        import torch
+        ip, il = _ptr_len(data)
+        n = C.c_size_t(0)
+        if out is None:
+            rc = self.L.sj_test_zstd_encode(self.h, ip, il, None, 0, C.byref(n))
+            if rc not in (OK, ERR_CAPACITY):
+                return rc, n.value, None
+            out = torch.empty(max(n.value, 1), dtype=torch.uint8, device=data.device)
+        rc = self.L.sj_test_zstd_encode(self.h, ip, il, out.data_ptr(), out.numel(), C.byref(n))
+        return rc, n.value, out[:n.value]
+
+    def zstd_decode(self, stream, want, out=None):
+        """test hook: the zstd frames `stream` (uint8 tensor) read as a block of `want` uncompressed bytes by the device
+        decoder, into `out` or a new tensor: (rc, the view of its `want` bytes or None)"""
+        import torch
+        ip, il = _ptr_len(stream)
+        if out is None:
+            out = torch.empty(max(want, 1), dtype=torch.uint8, device=stream.device)
+        got = C.c_size_t(0)
+        rc = self.L.sj_test_zstd_decode(self.h, ip, il, out.data_ptr(), want, C.byref(got))
         return rc, (out[:got.value] if rc == OK else None)
 
     def set_string_hash_bits(self, bits):
@@ -515,7 +544,8 @@ def ParseND(b, reuse=None, copy_strings=True, ctx=None):
 
 class Serializer:
     """parsed_serialize.go:44 Serializer, on the default context's device.  Blocks are uncompressed (CompressNone) unless
-    CompressMode(CompressFast) asks for S2 blocks, and strings are deduplicated exactly (first occurrence), so the stream
+    CompressMode asks for S2 (CompressFast), zstd tags with S2 message and values (CompressDefault) or zstd blocks
+    (CompressBest), and strings are deduplicated exactly (first occurrence), so the stream
     does not depend on copy_strings; the reference's Deserialize reads it."""
 
     def __init__(self, ctx=None):
@@ -523,11 +553,8 @@ class Serializer:
         self.mode = CompressNone
 
     def CompressMode(self, c):
-        """parsed_serialize.go:93 CompressMode: CompressNone or CompressFast; CompressDefault / CompressBest raise
-        SjError (SJ_ERR_UNSUPPORTED: zstd)"""
-        if c in (CompressDefault, CompressBest):
-            raise SjError(ERR_UNSUPPORTED)
-        if c not in (CompressNone, CompressFast):
+        """parsed_serialize.go:93 CompressMode: CompressNone, CompressFast, CompressDefault or CompressBest"""
+        if c not in (CompressNone, CompressFast, CompressDefault, CompressBest):
             raise ValueError("unknown compression mode")
         self.mode = c
 
@@ -556,8 +583,8 @@ class Serializer:
         return out.cpu().numpy().tobytes()
 
     def Deserialize(self, src):
-        """a ParsedJson from a v3 stream with uncompressed blocks, or S2 blocks in CompressFast mode (SJ_ERR_UNSUPPORTED for
-        zstd blocks, and for S2 blocks in CompressNone mode)"""
+        """a ParsedJson from a v3 stream with uncompressed blocks, S2 blocks outside CompressNone mode and zstd blocks in
+        CompressDefault / CompressBest mode (SJ_ERR_UNSUPPORTED for the others)"""
         return self._call(lambda ctx: self._deserialize(ctx, src))
 
     def _deserialize(self, ctx, src):

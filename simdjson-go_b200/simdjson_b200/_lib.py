@@ -22,7 +22,7 @@ EXPORTS = [
     "sj_stage1_launch", "sj_ctx_sync", "sj_event_record", "sj_event_elapsed_ms", "sj_kernel_launches",
     "sj_test_block_masks", "sj_test_geometry", "sj_test_finalize", "sj_test_flatten_bits", "sj_test_parse_strings",
     "sj_test_parse_numbers", "sj_count_where_device", "sj_parse_count_where", "sj_find_device", "sj_parse_find", "sj_marshal_device", "sj_parse_marshal", "sj_serialize_device", "sj_parse_serialize",
-    "sj_deserialize_device", "sj_test_set_string_hash_bits", "sj_ctx_set_compress_mode", "sj_test_s2_encode", "sj_test_s2_decode", "sj_test_stage2_internal", "sj_test_stage1_ctas", "sj_stream_create", "sj_stream_destroy",
+    "sj_deserialize_device", "sj_test_set_string_hash_bits", "sj_ctx_set_compress_mode", "sj_test_s2_encode", "sj_test_s2_decode", "sj_test_zstd_encode", "sj_test_zstd_decode", "sj_test_stage2_internal", "sj_test_stage1_ctas", "sj_stream_create", "sj_stream_destroy",
     "sj_stream_write", "sj_stream_close_input", "sj_stream_next", "sj_stream_release",
 ]
 STREAM_END, STREAM_EMPTY, STREAM_BUSY = 7, 8, 9
@@ -171,6 +171,10 @@ def load():
     L.sj_test_s2_encode.argtypes = [vp, vp, sz, vp, sz, szp]
     L.sj_test_s2_decode.restype = i32
     L.sj_test_s2_decode.argtypes = [vp, vp, sz, vp, sz, szp]
+    L.sj_test_zstd_encode.restype = i32
+    L.sj_test_zstd_encode.argtypes = [vp, vp, sz, vp, sz, szp]
+    L.sj_test_zstd_decode.restype = i32
+    L.sj_test_zstd_decode.argtypes = [vp, vp, sz, vp, sz, szp]
     L.sj_test_stage2_internal.restype = i32
     L.sj_test_stage2_internal.argtypes = [vp, C.POINTER(u32)]
     L.sj_test_stage1_ctas.restype = i32
