@@ -197,6 +197,9 @@ int sj_parse_count_where(sj_ctx* ctx, const uint8_t* msg, size_t len, uint32_t f
  *   SJ_FIND_KIND_ELEMENT  none               SJ_FIND_KIND_INT64   Iter.Int    (:629-661)
  *   SJ_FIND_KIND_UINT64   Iter.Uint (:679-712) SJ_FIND_KIND_FLOAT64 Iter.Float (:560-583)
  *   SJ_FIND_KIND_BOOL     Iter.Bool (:867-875) SJ_FIND_KIND_STRING  Iter.StringBytes (:741-749)
+ *   SJ_FIND_KIND_JSON     Element.Iter.MarshalJSON (:394-556): the element as compact JSON text, byte for byte what the
+ *                         reference writes (strings escaped like escapeBytes, floats like appendFloat); a scalar gives
+ *                         its own text ("abc", 12, true).  Its number is 7: 6 stays an unknown kind (SJ_ERR_ARGUMENT).
  * So the first member with the key decides, keys compare on their unescaped bytes, arrays are never entered, and a
  * root or intermediate value that is not an object is SJ_FIND_NOT_OBJECT, not SJ_FIND_NOT_FOUND.  Where amd64 Go and
  * CUDA's conversions differ the cell follows Go: Int() of a float of exactly 2^63 is math.MinInt64 (CVTTSD2SQ), Uint()
@@ -205,12 +208,20 @@ int sj_parse_count_where(sj_ctx* ctx, const uint8_t* msg, size_t len, uint32_t f
  * SJ_FIND_NOT_OBJECT "type ... found before object" / "value of key ... is not an object"; SJ_FIND_CONVERT the accessor's
  * error; SJ_FIND_CORRUPT any other error (or panic) of the reference on a malformed tape.  Tag (u8): the found element's
  * tag byte; index (i64): the tape index of its head word (-1 and tag 0 when nothing was found); value (8 bytes): int64,
- * uint64, the bits of a float64, 0 / 1 for BOOL, the byte length for STRING, 0 for ELEMENT and for cells not OK.
+ * uint64, the bits of a float64, 0 / 1 for BOOL, the byte length for STRING and JSON, 0 for ELEMENT and for cells not OK.
+ * A JSON cell is SJ_FIND_CONVERT when the element is TypeNone (the key's value is missing at the very end of a malformed
+ * tape: MarshalJSON's "no content queued in iterator"), and SJ_FIND_CORRUPT when its sub-tree, the words [index, index +
+ * its restricted tape length), fails the checks sj_marshal_device applies (tags, open / close links, string ranges,
+ * object keys, finite floats), or holds a root ('r') or nop ('N') word.  This is stricter than the reference's walk, as
+ * the whole-tape marshal is; the checks read the sub-tree alone, so a malformed region elsewhere on the tape leaves a
+ * cell whose own sub-tree is well formed unchanged.
  * Layout, path-major with a row stride of row_cap: cell (p, r) of status / tag / index / value is at p * row_cap + r;
- * STRING path s (counting STRING paths only, in path order) has str_offsets[s * (row_cap + 1) + r], r = 0 .. rows, into
- * str_bytes, so row r's bytes are [off[r], off[r + 1]) (with no rows, the one entry 0 is written when str_offsets is given).
+ * STRING and JSON path s (counting those paths only, in path order) has str_offsets[s * (row_cap + 1) + r], r = 0 ..
+ * rows, into str_bytes, so row r's bytes are [off[r], off[r + 1]) (with no rows, the one entry 0 is written when
+ * str_offsets is given).  A call without JSON paths writes what it wrote before they existed.
  * Limits: 1 to 64 paths, 0 to 32 segments each, 16 KiB of segment bytes in all; else SJ_ERR_ARGUMENT.  A tape longer
- * than 2^32 - 1 words returns SJ_ERR_TOO_LARGE.  *rows and *str_bytes are exact even on SJ_ERR_CAPACITY (rows > row_cap
+ * than 2^32 - 1 words returns SJ_ERR_TOO_LARGE, and so does a JSON path whose cells cover more than SJ_MAX_MARSHAL_TAPE
+ * tape words in all (only a malformed tape's cells can overlap, so on any other tape this is within the tape).  *rows and *str_bytes are exact even on SJ_ERR_CAPACITY (rows > row_cap
  * or str_bytes > str_cap), when nothing is written; out may be NULL to ask for the sizes.
  * sj_find_device: message, tape, strings and out in device memory, with their lengths (every read stays inside them).
  * On the tape this context's last parse left in HBM the rows are stage 2's root list, until the next parse or an
@@ -230,6 +241,7 @@ int sj_parse_count_where(sj_ctx* ctx, const uint8_t* msg, size_t len, uint32_t f
 #define SJ_FIND_KIND_FLOAT64 3
 #define SJ_FIND_KIND_BOOL 4
 #define SJ_FIND_KIND_STRING 5
+#define SJ_FIND_KIND_JSON 7
 typedef struct {
     const uint8_t* segments;   /* the key segments laid end to end (host memory) */
     const uint32_t* seg_lens;  /* n_segments lengths */
@@ -260,7 +272,8 @@ int sj_parse_find(sj_ctx* ctx, const uint8_t* msg, size_t len, uint32_t flags, c
  * tape is checked (tags, links of opens / closes / roots, string ranges, object keys, finite floats): a malformed one
  * returns SJ_ERR_ARGUMENT and nothing outside the three inputs is read.  *out_len = bytes of the text, exact even on
  * SJ_ERR_CAPACITY, when nothing is written.  A tape of length 0 gives 0 bytes.  Tapes longer than SJ_MAX_MARSHAL_TAPE
- * words (the passes keep int32 depths and parents per word) return SJ_ERR_TOO_LARGE.
+ * words (the passes keep int32 depths and parents per word) return SJ_ERR_TOO_LARGE.  The same bound holds for the
+ * words one SJ_FIND_KIND_JSON path's cells cover in sj_find_device / sj_parse_find.
  * sj_parse_marshal: HOST message in, parse and marshal on the device, only the text is copied to `out` (host memory);
  * parse errors return the parse codes.
  */

@@ -76,8 +76,9 @@ struct sj_ctx {
     DevBuf tape, strings;  // device outputs for the host-buffer API
     // tape consumers (tape.cuh and its users), each alive within one call only: the call's arguments (countWhere's
     // needles, the find's paths), the scratch of its passes, the Serializer's string dedup, the root list of a foreign
-    // tape and the scan that finds it, and the output of an sj_parse_* call before its copy to the host
-    DevBuf args, scratch, sz_tab, tc_roots, tc_scan, staging;
+    // tape and the scan that finds it, the output of an sj_parse_* call before its copy to the host, and the per-word
+    // passes of the find's JSON paths (find_json.cuh)
+    DevBuf args, scratch, sz_tab, tc_roots, tc_scan, staging, fj;
     uint32_t sz_hash_bits = 0;  // test hook: keep only this many bits of the dedup hash (0 = all)
     // the Serializer's compress mode (SJ_COMPRESS_*) and, within one call, the S2 and zstd codecs' buffers (s2.cuh,
     // zstd.cuh): the uncompressed stream and the encoders' chunk slots; the chunk, frame and block lists and the

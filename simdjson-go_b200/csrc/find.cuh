@@ -14,10 +14,13 @@
 // Rows are the roots in tape order: stage 2's root list for the tape the context just built, else KC1a / KC1b
 // (tape.cuh), as for countWhere.
 //   KF3 fd_walk         one thread per (path, row), path-major, the path's segments staged in shared memory; the cell's
-//       status, tag, head index and converted value into scratch, a STRING cell's length into `slen`
+//       status, tag, head index and converted value into scratch, a STRING cell's length into `slen`, a JSON cell's
+//       tape words into `jlen`
+//   (JSON paths: the passes of find_json.cuh write each JSON cell's text length into `slen`, `val` and its status)
 //   KF4 fd_len_reduce   per-tile sums of `slen` (scan_groups_kernel twice)
-//   KF5 fd_emit         the columns into the caller's buffers: string offsets from the scan and the bytes (strings
-//       longer than FD_SHORT by their whole warp), and the fixed-size columns with the caller's row stride
+//   KF5 fd_emit         the columns into the caller's buffers: STRING and JSON offsets from the scan and the STRING
+//       bytes (strings longer than FD_SHORT by their whole warp), and the fixed-size columns with the caller's row stride
+//   (JSON paths: find_json.cuh's KJ6 writes the text behind KF5's offsets)
 #pragma once
 #include "common.cuh"
 #include "tape.cuh"
@@ -29,12 +32,13 @@ constexpr uint64_t FD_SHORT = 32;   // longer strings are copied by their whole 
 
 // cell status (SJ_FIND_*) and path kind (SJ_FIND_KIND_*)
 enum : uint32_t { FD_OK = 0, FD_NOT_FOUND = 1, FD_NOT_OBJECT = 2, FD_CONVERT = 3, FD_CORRUPT = 4 };
-enum : uint32_t { FD_ELEMENT = 0, FD_INT64 = 1, FD_UINT64 = 2, FD_FLOAT64 = 3, FD_BOOL = 4, FD_STRING = 5 };
+enum : uint32_t { FD_ELEMENT = 0, FD_INT64 = 1, FD_UINT64 = 2, FD_FLOAT64 = 3, FD_BOOL = 4, FD_STRING = 5, FD_JSON = 7 };
 
 struct FdPath {
     uint32_t seg0, nseg;  // its segments: segs[seg0 .. seg0 + nseg)
     uint32_t kind;
-    uint32_t sidx;        // STRING paths: index among them
+    uint32_t sidx;        // STRING and JSON paths: index among them (their variable-length column)
+    uint32_t jidx;        // JSON paths: index among them
 };
 struct FdSeg {
     uint32_t off, len;    // bytes [off, off + len) of the segment bytes
@@ -52,7 +56,8 @@ struct FindParams {
     uint8_t* tag;
     int64_t* idx;
     uint64_t* val;
-    uint64_t* slen;          // STRING cells: bytes of the string (0 unless OK), at sidx * rows + r
+    uint64_t* slen;          // STRING and JSON cells: bytes of the string or text (0 unless OK), at sidx * rows + r
+    uint64_t* jlen;          // JSON cells: tape words of the found element (0 unless found), at jidx * rows + r
 };
 
 // the Iter fields the walk uses (parsed_json.go:180-195); n = length of its restricted tape
@@ -345,19 +350,25 @@ __global__ void __launch_bounds__(FD_THREADS) fd_walk_kernel(const FindParams p)
     int64_t idx = -1;
     uint64_t val = 0;
     const uint8_t* s = nullptr;
+    uint64_t words = 0;
     if (st == FD_OK && fresh) {
         st = path.kind == FD_ELEMENT ? FD_OK : FD_CONVERT;  // a fresh Element: Type None, a zero Iter
     } else if (st == FD_OK) {
         tag = e.t;
         idx = (int64_t)e.off - 1;
-        st = fd_convert(p, e, path.kind, &val, &s);
-        if (st != FD_OK) val = 0;
+        if (path.kind == FD_JSON) {
+            words = e.n - (uint64_t)idx;  // MarshalJSON's scope: the element's restricted tape [head, n)
+        } else {
+            st = fd_convert(p, e, path.kind, &val, &s);
+            if (st != FD_OK) val = 0;
+        }
     }
     p.st[q] = (uint8_t)st;
     p.tag[q] = (uint8_t)tag;
     p.idx[q] = idx;
     p.val[q] = val;
-    if (path.kind == FD_STRING) p.slen[(uint64_t)path.sidx * p.roots.n + r] = val;
+    if (path.kind == FD_STRING || path.kind == FD_JSON) p.slen[(uint64_t)path.sidx * p.roots.n + r] = val;
+    if (path.kind == FD_JSON) p.jlen[(uint64_t)path.jidx * p.roots.n + r] = words;
 }
 
 // KF4: per-tile sums of slen
@@ -377,7 +388,8 @@ struct FindEmit {
     uint64_t rows, row_cap;
     uint32_t n_paths, n_str;
     uint32_t str_ntiles;
-    uint8_t str_path[64];        // the path of every STRING path index
+    uint8_t str_path[64];        // the path of every STRING and JSON path index
+    uint64_t str_json;           // bit s: column s is a JSON path's (its bytes come from KJ6)
     const uint8_t* st;
     const uint8_t* tag;
     const int64_t* idx;
@@ -420,24 +432,27 @@ __global__ void __launch_bounds__(TAPE_THREADS) fd_emit_kernel(const FindEmit p)
         const uint64_t off = carry + block_exclusive_scan(MSum{len}, total).v;
         carry += total.v;
         const uint8_t* s = nullptr;
+        uint64_t copy = 0;  // bytes of a STRING cell
         if (k < n) {
             const uint64_t si = k / p.rows, r = k - si * p.rows;
             int64_t* col = p.o_off + si * (p.row_cap + 1);
             col[r] = (int64_t)off;
             if (r + 1 == p.rows) col[p.rows] = (int64_t)(off + len);
-            if (len)  // an OK cell: its head word is a string whose range was checked by KF3
+            if (len && !(p.str_json >> si & 1)) {  // an OK cell: its head word is a string whose range was checked by KF3
                 s = tape_string_ptr(p.t, p.t.tape[p.idx[(uint64_t)p.str_path[si] * p.rows + r]]);
+                copy = len;
+            }
         }
         uint8_t* d = p.o_bytes + off;
-        if (len <= FD_SHORT)
-            for (uint64_t b = 0; b < len; b++) d[b] = s[b];
-        uint32_t m = __ballot_sync(FULL, len > FD_SHORT);
+        if (copy <= FD_SHORT)
+            for (uint64_t b = 0; b < copy; b++) d[b] = s[b];
+        uint32_t m = __ballot_sync(FULL, copy > FD_SHORT);
         while (m) {
             const int src = __ffs(m) - 1;
             m &= m - 1;
             const uint8_t* ws = reinterpret_cast<const uint8_t*>(__shfl_sync(FULL, reinterpret_cast<unsigned long long>(s), src));
             uint8_t* wd = reinterpret_cast<uint8_t*>(__shfl_sync(FULL, reinterpret_cast<unsigned long long>(d), src));
-            const uint64_t wl = __shfl_sync(FULL, len, src);
+            const uint64_t wl = __shfl_sync(FULL, copy, src);
             for (uint64_t b = lane; b < wl; b += 32) wd[b] = ws[b];
         }
     }

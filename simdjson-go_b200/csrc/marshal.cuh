@@ -44,20 +44,29 @@ __global__ void __launch_bounds__(MJ_THREADS) mj_depth_kernel(const uint64_t* ta
     }
 }
 
-// KM3: F per word; fbits = parity of F's in-tile exclusive prefix, tile_f = F's count per tile
-__global__ void __launch_bounds__(MJ_THREADS) mj_keys_kernel(const uint64_t* tape, uint64_t n, const int32_t* depth,
-                                                            const int32_t* par, uint32_t* fbits, MSum* tile_f) {
+// KM3's words of a whole tape: F(i) = 1 for a non-close head whose parent is '{'
+struct MjTapeWords {
+    const uint64_t* tape;
+    uint64_t n;
+    __device__ __forceinline__ bool f(uint64_t i, const int32_t* depth, const int32_t* par) const {
+        if (i >= n || depth[i] == MJ_PAYLOAD || mj_is_close(tape[i], i)) return false;
+        const int32_t p = par[i];
+        return p >= 0 && (tape[p] >> 56) == '{';
+    }
+};
+
+// KM3: F per word; fbits = parity of F's in-tile exclusive prefix, tile_f = F's count per tile.  W is MjTapeWords, or
+// the cells' virtual word space of the find's JSON paths (find_json.cuh)
+template <class W>
+__global__ void __launch_bounds__(MJ_THREADS) mj_keys_kernel(const W words, const int32_t* depth, const int32_t* par,
+                                                            uint32_t* fbits, MSum* tile_f) {
     __shared__ uint32_t cnt[MJ_ROUNDS * 32];
     const uint32_t lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
     uint32_t b[MJ_ROUNDS];
 #pragma unroll
     for (int r = 0; r < MJ_ROUNDS; r++) {
         const uint64_t i = (uint64_t)blockIdx.x * MJ_TILE + (uint64_t)r * MJ_THREADS + threadIdx.x;
-        bool f = false;
-        if (i < n && depth[i] != MJ_PAYLOAD && !mj_is_close(tape[i], i)) {
-            const int32_t p = par[i];
-            f = p >= 0 && (tape[p] >> 56) == '{';
-        }
+        const bool f = words.f(i, depth, par);
         b[r] = __ballot_sync(FULL, f);
         if (lane == 0) cnt[r * 32 + warp] = __popc(b[r]);
     }
@@ -123,33 +132,47 @@ struct MjItem {
     bool long_str;
 };
 
-// What head i writes, after the checks of a foreign tape: false = malformed.  Every read stays inside the tape, the
-// string buffer or the message.
-__device__ bool mj_item(const MarshalParams& p, uint64_t i, MjItem& it) {
+// The words [lo, hi) of the value a word belongs to (the whole tape, or one JSON cell of the find), and d = its tape
+// index - its index in the per-word arrays (depth, par, fbits)
+struct MjSpan {
+    uint64_t lo, hi;
+    int64_t d;
+};
+
+// What head i writes, after the checks of a foreign tape: false = malformed.  Every read stays inside the span, the
+// string buffer or the message.  CELL: the span is one element's sub-tree, whose head alone sits at its top level and
+// writes no separator, and which holds no root word.
+template <bool CELL>
+__device__ bool mj_item(const MarshalParams& p, uint64_t i, const MjSpan& s, MjItem& it) {
     const uint64_t w = p.t.tape[i];
     const uint32_t t = (uint32_t)(w >> 56);
     const uint64_t v = w & TAPE_VALUE_MASK;
-    const int32_t pp = p.par[i];
+    const int32_t pv = p.par[i - s.d];
+    const int64_t pp = pv < 0 ? -1 : (int64_t)pv + s.d;  // the parent's tape index
     uint32_t pt = 0;
     if (pp >= 0) {
         const uint64_t pw = p.t.tape[pp];
         pt = (uint32_t)(pw >> 56);
         if (!(pt == '{' || pt == '[' || (pt == 'r' && (pw & TAPE_VALUE_MASK) > (uint64_t)pp))) return false;  // parent is no open
     }
-    if (t == 'r' && v > i) return pp < 0;  // a root open writes nothing and sits at the top level
-    if (pp < 0) return false;
+    if (CELL) {
+        if (t == 'r' || (pp < 0 && i != s.lo)) return false;
+    } else {
+        if (t == 'r' && v > i) return pp < 0;  // a root open writes nothing and sits at the top level
+        if (pp < 0) return false;
+    }
     if (t == '}' || t == ']' || t == 'r') {  // close: its parent is its open, and the two point at each other
         const uint32_t want = t == '}' ? '{' : t == ']' ? '[' : 'r';
         if (pt != want || v != (uint64_t)pp || (p.t.tape[pp] & TAPE_VALUE_MASK) != i + 1) return false;
-        if (t == '}' && mj_x(p, i) != mj_x(p, pp + 1)) return false;  // an object ends behind a key
+        if (t == '}' && mj_x(p, i - s.d) != mj_x(p, pp + 1 - s.d)) return false;  // an object ends behind a key
         it.tag = t;
         if (t == 'r') {
-            it.sep = i + 1 < p.t.n ? '\n' : 0;
+            it.sep = i + 1 < s.hi ? '\n' : 0;
         } else {  // a container inside a container: the ',' in front of its next sibling goes behind the close
-            const int32_t gp = p.par[pp];
-            const uint32_t gt = gp >= 0 ? (uint32_t)(p.t.tape[gp] >> 56) : 0;
+            const int32_t gv = p.par[pp - s.d];
+            const uint32_t gt = gv >= 0 ? (uint32_t)(p.t.tape[gv + s.d] >> 56) : 0;
             if (gt == '{' || gt == '[') {
-                if (i + 1 >= p.t.n) return false;
+                if (i + 1 >= s.hi) return false;
                 const uint32_t nt = (uint32_t)(p.t.tape[i + 1] >> 56);
                 if (nt != '}' && nt != ']') it.sep = ',';
             }
@@ -157,11 +180,11 @@ __device__ bool mj_item(const MarshalParams& p, uint64_t i, MjItem& it) {
         it.len = (t != 'r') + (it.sep != 0);
         return true;
     }
-    const bool key = pt == '{' && mj_x(p, i) == mj_x(p, pp + 1);
+    const bool key = pt == '{' && mj_x(p, i - s.d) == mj_x(p, pp + 1 - s.d);
     if (key && t != '"') return false;
     uint64_t end = i + 1;  // the word behind the value
     if (tape_value_tag(t)) {
-        if (i + 1 >= p.t.n) return false;
+        if (i + 1 >= s.hi) return false;
         const uint64_t pl = p.t.tape[i + 1];
         end = i + 2;
         it.payload = pl;
@@ -195,8 +218,8 @@ __device__ bool mj_item(const MarshalParams& p, uint64_t i, MjItem& it) {
     it.tag = t;
     if (key) {
         it.sep = ':';
-    } else if (pt != 'r') {
-        if (end <= i || end >= p.t.n) return false;
+    } else if (pt == '{' || pt == '[') {  // (not behind a root's value, nor a cell's head)
+        if (end <= i || end >= s.hi) return false;
         const uint32_t nt = (uint32_t)(p.t.tape[end] >> 56);
         if (nt != '}' && nt != ']') it.sep = ',';
     }
@@ -204,8 +227,10 @@ __device__ bool mj_item(const MarshalParams& p, uint64_t i, MjItem& it) {
     return true;
 }
 
-// word i of the tape: its item (tag 0 for value words) and, with the whole warp, a long string's escaped length
-__device__ __forceinline__ bool mj_load(const MarshalParams& p, uint64_t i, MjItem& it, uint64_t& body) {
+// word i of the tape (when `in`): its item (tag 0 for value words) and, with the whole warp, a long string's escaped
+// length
+template <bool CELL>
+__device__ __forceinline__ bool mj_load(const MarshalParams& p, bool in, uint64_t i, const MjSpan& s, MjItem& it, uint64_t& body) {
     it.len = 0;
     it.tag = 0;
     it.sep = 0;
@@ -213,7 +238,7 @@ __device__ __forceinline__ bool mj_load(const MarshalParams& p, uint64_t i, MjIt
     it.s = nullptr;
     it.slen = 0;
     bool ok = true;
-    if (i < p.t.n && p.depth[i] != MJ_PAYLOAD) ok = mj_item(p, i, it);
+    if (in && p.depth[i - s.d] != MJ_PAYLOAD) ok = mj_item<CELL>(p, i, s, it);
     if (!ok) it.long_str = false;
     body = 0;
     uint32_t m = __ballot_sync(FULL, it.long_str);
@@ -243,7 +268,7 @@ __global__ void __launch_bounds__(MJ_THREADS) mj_measure_kernel(const MarshalPar
         const uint64_t i = (uint64_t)blockIdx.x * MJ_TILE + (uint64_t)r * MJ_THREADS + threadIdx.x;
         MjItem it;
         uint64_t body;
-        bad |= !mj_load(p, i, it, body);
+        bad |= !mj_load<false>(p, i < p.t.n, i, MjSpan{0, p.t.n, 0}, it, body);
         acc += it.len;
     }
     if (blockIdx.x == 0 && threadIdx.x == 0 && (p.h_total->d1 != 0 || hagg_out(*p.h_total, 1) != 1))
@@ -265,60 +290,70 @@ __device__ __forceinline__ void mj_put(uint8_t* o, const char* s, uint32_t n) {
     for (uint32_t k = 0; k < n; k++) o[k] = (uint8_t)s[k];
 }
 
+// the bytes of item `it` at o, but for a long string's body (mj_put_long)
+__device__ __forceinline__ void mj_put_item(const MjItem& it, uint64_t body, uint8_t* o) {
+    switch (it.tag) {
+    case '"':
+        o[0] = '"';
+        if (!it.long_str) {
+            body = 0;
+            for (uint64_t k = 0; k < it.slen; k++) body += fmt_escape(it.s[k], o + 1 + body);
+        }
+        o[1 + body] = '"';
+        break;
+    case 'l': fmt_i64<true>((int64_t)it.payload, o); break;
+    case 'u': fmt_u64<true>(it.payload, o); break;
+    case 'd': fmt_double<true>(it.payload, o); break;
+    case 't': mj_put(o, "true", 4); break;
+    case 'f': mj_put(o, "false", 5); break;
+    case 'n': mj_put(o, "null", 4); break;
+    case '{': case '}': case '[': case ']': o[0] = (uint8_t)it.tag; break;
+    default: break;
+    }
+    if (it.sep) o[it.len - 1] = (uint8_t)it.sep;
+}
+
+// long strings: the warp escapes 32 bytes at a time, each lane one byte at its place in the scan of the lengths; the
+// whole warp calls it, o is where the item of each lane goes
+__device__ __forceinline__ void mj_put_long(const MjItem& it, uint8_t* o) {
+    const uint32_t lane = threadIdx.x & 31;
+    uint32_t m = __ballot_sync(FULL, it.long_str);
+    while (m) {
+        const int src = __ffs(m) - 1;
+        m &= m - 1;
+        const uint8_t* s = reinterpret_cast<const uint8_t*>(__shfl_sync(FULL, reinterpret_cast<unsigned long long>(it.s), src));
+        const uint64_t sl = __shfl_sync(FULL, it.slen, src);
+        uint8_t* d = reinterpret_cast<uint8_t*>(__shfl_sync(FULL, reinterpret_cast<unsigned long long>(o + 1), src));
+        for (uint64_t k0 = 0; k0 < sl; k0 += 32) {
+            const uint64_t k = k0 + lane;
+            const uint8_t c = k < sl ? s[k] : 0;
+            const uint32_t e = k < sl ? fmt_escaped_len(c) : 0;
+            uint32_t inc = e;
+#pragma unroll
+            for (int dd = 1; dd < 32; dd <<= 1) {
+                const uint32_t t = __shfl_up_sync(FULL, inc, dd);
+                if ((int)lane >= dd) inc += t;
+            }
+            if (e) fmt_escape(c, d + inc - e);
+            d += __shfl_sync(FULL, inc, 31);
+        }
+    }
+}
+
 // KM5: every word's bytes at the exclusive scan of the lengths
 __global__ void __launch_bounds__(MJ_THREADS) mj_emit_kernel(const MarshalParams p) {
-    const uint32_t lane = threadIdx.x & 31;
     uint64_t carry = tile_prefix(p.len_tile_pre, p.len_grp_pre, blockIdx.x).v;
     for (int r = 0; r < MJ_ROUNDS; r++) {
         const uint64_t i = (uint64_t)blockIdx.x * MJ_TILE + (uint64_t)r * MJ_THREADS + threadIdx.x;
         MjItem it;
         uint64_t body;
-        mj_load(p, i, it, body);
+        mj_load<false>(p, i < p.t.n, i, MjSpan{0, p.t.n, 0}, it, body);
         MSum total;
         const uint64_t off = carry + block_exclusive_scan(MSum{it.len}, total).v;
         carry += total.v;
         uint8_t* o = p.out + off;
-        switch (it.tag) {
-        case '"':
-            o[0] = '"';
-            if (!it.long_str) {
-                body = 0;
-                for (uint64_t k = 0; k < it.slen; k++) body += fmt_escape(it.s[k], o + 1 + body);
-            }
-            o[1 + body] = '"';
-            break;
-        case 'l': fmt_i64<true>((int64_t)it.payload, o); break;
-        case 'u': fmt_u64<true>(it.payload, o); break;
-        case 'd': fmt_double<true>(it.payload, o); break;
-        case 't': mj_put(o, "true", 4); break;
-        case 'f': mj_put(o, "false", 5); break;
-        case 'n': mj_put(o, "null", 4); break;
-        case '{': case '}': case '[': case ']': o[0] = (uint8_t)it.tag; break;
-        default: break;
-        }
-        if (it.sep) o[it.len - 1] = (uint8_t)it.sep;
-        // long strings: the warp escapes 32 bytes at a time, each lane one byte at its place in the scan of the lengths
-        uint32_t m = __ballot_sync(FULL, it.long_str);
-        while (m) {
-            const int src = __ffs(m) - 1;
-            m &= m - 1;
-            const uint8_t* s = reinterpret_cast<const uint8_t*>(__shfl_sync(FULL, reinterpret_cast<unsigned long long>(it.s), src));
-            const uint64_t sl = __shfl_sync(FULL, it.slen, src);
-            uint8_t* d = reinterpret_cast<uint8_t*>(__shfl_sync(FULL, reinterpret_cast<unsigned long long>(o + 1), src));
-            for (uint64_t k0 = 0; k0 < sl; k0 += 32) {
-                const uint64_t k = k0 + lane;
-                const uint8_t c = k < sl ? s[k] : 0;
-                const uint32_t e = k < sl ? fmt_escaped_len(c) : 0;
-                uint32_t inc = e;
-#pragma unroll
-                for (int dd = 1; dd < 32; dd <<= 1) {
-                    const uint32_t t = __shfl_up_sync(FULL, inc, dd);
-                    if ((int)lane >= dd) inc += t;
-                }
-                if (e) fmt_escape(c, d + inc - e);
-                d += __shfl_sync(FULL, inc, 31);
-            }
-        }
+        mj_put_item(it, body, o);
+        mj_put_long(it, o);
     }
 }
 

@@ -25,6 +25,7 @@
 #include "tape.cuh"
 #include "consume.cuh"
 #include "find.cuh"
+#include "find_json.cuh"
 #include "marshal.cuh"
 #include "serialize.cuh"
 #include "zstd.cuh"
@@ -213,7 +214,7 @@ extern "C" void sj_ctx_destroy(sj_ctx* c) {
     exchange_release(c);
     DevBuf* bufs[] = {&c->msg,     &c->idx,      &c->desc,     &c->result, &c->s2a,     &c->s2b,    &c->s2c,
                       &c->tape,    &c->strings,  &c->test_in,  &c->test_out, &c->test_aux, &c->args, &c->scratch,
-                      &c->sz_tab,  &c->tc_roots, &c->tc_scan,  &c->staging, &c->s2_raw, &c->s2_slots, &c->s2_list,
+                      &c->sz_tab,  &c->tc_roots, &c->tc_scan,  &c->staging, &c->fj, &c->s2_raw, &c->s2_slots, &c->s2_list,
                       &c->s2_out,  &c->zx_seq,   &c->zx_src};
     for (DevBuf* b : bufs) b->release();
     if (c->host_result) cudaFreeHost(c->host_result);

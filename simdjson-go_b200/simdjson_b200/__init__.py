@@ -12,7 +12,7 @@ import numpy as np
 from . import _lib
 from ._lib import (COMPRESS_BEST, COMPRESS_DEFAULT, COMPRESS_FAST, COMPRESS_NONE, ERR_CAPACITY, ERR_STAGE1, ERR_STAGE2,
                    ERR_UNSUPPORTED, FIND_CONVERT, FIND_CORRUPT, FIND_KIND_BOOL,
-                   FIND_KIND_ELEMENT, FIND_KIND_FLOAT64, FIND_KIND_INT64, FIND_KIND_STRING, FIND_KIND_UINT64,
+                   FIND_KIND_ELEMENT, FIND_KIND_FLOAT64, FIND_KIND_INT64, FIND_KIND_JSON, FIND_KIND_STRING, FIND_KIND_UINT64,
                    FIND_NOT_FOUND, FIND_NOT_OBJECT, FIND_OK, FLAG_COPY_STRINGS, FLAG_NDJSON, OK, SjError, Stage1Info)
 
 JSONVALUEMASK = 0xFF_FFFF_FFFF_FFFF  # parsed_json.go:26
@@ -130,8 +130,8 @@ class Context:
         """parseMessage + ForEach(FindElement(path...) + the accessor of each kind) (ndjson_test.go:294-315) with the tape
         left in HBM: (rc, rows, columns).  `paths` is a list of key paths (each a list of byte strings), `kinds` the
         FIND_KIND_* of each.  columns[p] is a FindColumn of numpy arrays (status, tag, index, value, offsets, data):
-        `value` is int64 / uint64 / float64 by kind (int64 for ELEMENT, BOOL and STRING, where it is the length); a
-        STRING column's row r is data[offsets[r]:offsets[r + 1]].  Only the columns are copied back; on a parse error
+        `value` is int64 / uint64 / float64 by kind (int64 for ELEMENT, BOOL, STRING and JSON, where it is the length); a
+        STRING or JSON column's row r is data[offsets[r]:offsets[r + 1]] (JSON: the element's MarshalJSON text).  Only the columns are copied back; on a parse error
         rows is 0 and columns is None."""
         m = _as_u8(msg)
         flags = (FLAG_NDJSON if ndjson else 0) | (FLAG_COPY_STRINGS if copy_strings else 0)
@@ -141,7 +141,7 @@ class Context:
         # STRING path, guessed at its size -- else once more at the exact sizes
         row_cap = int(np.count_nonzero(m == 10)) + 1 if ndjson else 1
         str_cap = m.size + 64
-        n_str = sum(k == FIND_KIND_STRING for k in kinds)
+        n_str = sum(k in (FIND_KIND_STRING, FIND_KIND_JSON) for k in kinds)
         for _ in range(2):
             cols = (np.empty((len(paths), row_cap), np.uint8), np.empty((len(paths), row_cap), np.uint8),
                     np.empty((len(paths), row_cap), np.int64), np.empty((len(paths), row_cap), np.uint64),
@@ -161,7 +161,7 @@ class Context:
     def find_device(self, tape, strings, message, paths, kinds, out=None):
         """ForEach + FindElement + accessors over a tape already on this context's device (torch tensors as for
         marshal_device).  `out` (optional) is a tuple of tensors (status u8 [P, R], tag u8 [P, R], index i64 [P, R],
-        value i64 [P, R], str_offsets i64 [S, R + 1], str_bytes u8 [B]) for P paths, S of them STRING, R >= rows;
+        value i64 [P, R], str_offsets i64 [S, R + 1], str_bytes u8 [B]) for P paths, S of them STRING or JSON, R >= rows;
         without it they are allocated at the exact sizes.  Returns (rc, rows, columns): columns[p] is a FindColumn of
         tensor views (value viewed as float64 for FLOAT64 and uint64 for UINT64), or None unless rc is OK.  rc is
         SJ_ERR_CAPACITY when `out` is too small (rows and the byte total are still exact, in `rows` and nothing written)."""
@@ -171,7 +171,7 @@ class Context:
         mp, ml = _ptr_len(message)
         tp, tl = _ptr_len(tape)
         rows, nbytes = C.c_size_t(0), C.c_size_t(0)
-        n_str = sum(k == FIND_KIND_STRING for k in kinds)
+        n_str = sum(k in (FIND_KIND_STRING, FIND_KIND_JSON) for k in kinds)
         if out is None:
             rc = self.L.sj_find_device(self.h, mp, ml, tp, tl, sp, sl, cpaths, len(paths), None, C.byref(rows), C.byref(nbytes))
             if rc not in (OK, ERR_CAPACITY):
@@ -448,7 +448,7 @@ def _ptr_len(t):
 
 
 class FindColumn(tuple):
-    """one path's column: status, tag, index, value per row; offsets / data for STRING (else None)"""
+    """one path's column: status, tag, index, value per row; offsets / data for STRING and JSON (else None)"""
     __slots__ = ()
     _fields = ("status", "tag", "index", "value", "offsets", "data")
 
@@ -489,7 +489,7 @@ def _find_columns(out, rows, kinds, view):
     for p, k in enumerate(kinds):
         dt = np.float64 if k == FIND_KIND_FLOAT64 else np.uint64 if k == FIND_KIND_UINT64 else np.int64
         o = d = None
-        if k == FIND_KIND_STRING:
+        if k in (FIND_KIND_STRING, FIND_KIND_JSON):
             o, d, s = offs[s, :rows + 1], data, s + 1
         cols.append(FindColumn(status[p, :rows], tag[p, :rows], index[p, :rows], view(value[p, :rows], dt), o, d))
     return cols

@@ -29,6 +29,7 @@ STREAM_END, STREAM_EMPTY, STREAM_BUSY = 7, 8, 9
 # sj_find_device / sj_parse_find: cell statuses and path kinds
 FIND_OK, FIND_NOT_FOUND, FIND_NOT_OBJECT, FIND_CONVERT, FIND_CORRUPT = range(5)
 FIND_KIND_ELEMENT, FIND_KIND_INT64, FIND_KIND_UINT64, FIND_KIND_FLOAT64, FIND_KIND_BOOL, FIND_KIND_STRING = range(6)
+FIND_KIND_JSON = 7  # (6 is no kind)
 # Serializer.CompressMode (sj_ctx_set_compress_mode)
 COMPRESS_NONE, COMPRESS_FAST, COMPRESS_DEFAULT, COMPRESS_BEST = range(4)
 FIND_MAX_PATHS, FIND_MAX_SEGMENTS, FIND_MAX_SEGMENT_BYTES = 64, 32, 16384

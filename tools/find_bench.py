@@ -7,6 +7,12 @@ ParseND'd into HBM, then ForEach + FindElement with 1, 4 and 16 paths (every key
   min_bytes          the least the algorithm moves: the tape read once, the string bytes read and written, and the
                      columns written (18 bytes per cell, 8 per STRING offset); min_gbs = min_bytes / find time
   host rates         sj_parse_find, sj_parse and sj_parse_count_where host to host, wall clock, GB/s of input
+Then one JSON line per JSON-cell workload (SJ_FIND_KIND_JSON), each beside sj_marshal_device of the same tape:
+  K0 batch          ["Fine"] and ["Make"] as JSON against the same paths as STRING
+  twitter NDJSON    twitter.json's statuses one per line, repeated to --mib: ["user"], ["entities"], and both
+  one cell          {"a": [twitter.json x K]} at --mib: the one cell of ["a"]
+  json_ms / string_ms / marshal_ms, launches per call, and min_bytes (the tape words the cells cover read once, the
+  text written, the columns) over json_ms as a fraction of 3.35 TB/s
 The card's name and power limit are read in the same run.
 usage: python tools/find_bench.py [--mib 512] [--calls 10] [--warmup 3]"""
 import argparse
@@ -155,6 +161,99 @@ def main():
             "card": name, "power_limit_w": plimit}), flush=True)
         del out_t, h_cols, h_tape, h_str
         torch.cuda.empty_cache()
+
+    def find_call(d_m, mlen, d_t, tw, d_s, slen, paths, kinds):
+        """a timed sj_find_device over a device tape into exact-size columns: (seconds, launches, rows, bytes, covered words)"""
+        cp, keep = _find_paths(paths, kinds)
+        rows, nbytes = C.c_size_t(0), C.c_size_t(0)
+        args_ = (ctx.h, d_m.data_ptr(), mlen, d_t.data_ptr(), tw, d_s.data_ptr(), slen, cp, len(paths))
+        assert L.sj_find_device(*args_, None, C.byref(rows), C.byref(nbytes)) in (0, _lib.ERR_CAPACITY)
+        R, k, ns = rows.value, len(paths), sum(x in (_lib.FIND_KIND_STRING, _lib.FIND_KIND_JSON) for x in kinds)
+        out_t = (torch.empty((k, R), dtype=torch.uint8, device=dev), torch.empty((k, R), dtype=torch.uint8, device=dev),
+                 torch.empty((k, R), dtype=torch.int64, device=dev), torch.empty((k, R), dtype=torch.int64, device=dev),
+                 torch.empty((ns, R + 1), dtype=torch.int64, device=dev), torch.empty(max(nbytes.value, 1), dtype=torch.uint8, device=dev))
+        out = _lib.FindOut(*(t.data_ptr() for t in out_t), R, nbytes.value)
+
+        def call():
+            assert L.sj_find_device(*args_, C.byref(out), C.byref(rows), C.byref(nbytes)) == 0
+
+        for _ in range(args.warmup):
+            call()
+        assert bool((out_t[0] == 0).all()), "a cell is not OK"
+        l0 = ctx.launches()
+        t = timed(call, args.calls)
+        launches = (ctx.launches() - l0) / args.calls
+        covered = 0
+        for p, kind in enumerate(kinds):
+            if kind == _lib.FIND_KIND_JSON:  # the element's words: head index to the next element's, from the tags
+                tags = (d_t[out_t[2][p]].view(torch.int64) >> 56) & 0xff
+                val = d_t[out_t[2][p]] & ((1 << 56) - 1)
+                scalar = torch.where((tags == ord('"')) | (tags == ord("l")) | (tags == ord("u")) | (tags == ord("d")), 2, 1)
+                covered += int(torch.where((tags == ord("{")) | (tags == ord("[")), val - out_t[2][p], scalar).sum())
+        return t, launches, R, nbytes.value, covered
+
+    def marshal_call(d_m, mlen, d_t, tw, d_s, slen):
+        n_out = C.c_size_t(0)
+        assert L.sj_marshal_device(ctx.h, d_m.data_ptr(), mlen, d_t.data_ptr(), tw, d_s.data_ptr(), slen, None, 0, C.byref(n_out)) == _lib.ERR_CAPACITY
+        o = torch.empty(n_out.value, dtype=torch.uint8, device=dev)
+
+        def call():
+            assert L.sj_marshal_device(ctx.h, d_m.data_ptr(), mlen, d_t.data_ptr(), tw, d_s.data_ptr(), slen, o.data_ptr(), o.numel(),
+                                       C.byref(n_out)) == 0
+
+        for _ in range(args.warmup):
+            call()
+        l0 = ctx.launches()
+        t = timed(call, args.calls)
+        return t, (ctx.launches() - l0) / args.calls, n_out.value
+
+    def json_rows(label, d_m, mlen, flags_, path_sets):
+        nonlocal d_tape, d_str
+        tl_, sl_ = C.c_size_t(0), C.c_size_t(0)
+        L.sj_bounds(mlen, C.byref(tl_), C.byref(sl_))
+        if tl_.value > d_tape.numel() or sl_.value > d_str.numel():
+            d_tape, d_str = None, None
+            torch.cuda.empty_cache()
+            d_tape = torch.empty(tl_.value, dtype=torch.int64, device=dev)
+            d_str = torch.empty(sl_.value, dtype=torch.uint8, device=dev)
+        assert L.sj_parse_device(ctx.h, d_m.data_ptr(), mlen, flags_, d_tape.data_ptr(), d_tape.numel(), C.byref(tl_),
+                                 d_str.data_ptr(), d_str.numel(), C.byref(sl_)) == 0
+        tw, slen = tl_.value, sl_.value
+        t_m, l_m, n_m = marshal_call(d_m, mlen, d_tape, tw, d_str, slen)
+        for paths in path_sets:
+            k = len(paths)
+            t_j, l_j, R, nb, covered = find_call(d_m, mlen, d_tape, tw, d_str, slen, paths, [_lib.FIND_KIND_JSON] * k)
+            row = {"input": label, "input_bytes": mlen, "tape_words": tw, "paths": [p[0].decode() for p in paths], "rows": R,
+                   "json_bytes_out": nb, "covered_words": covered, "json_ms": round(t_j * 1e3, 3), "launches_per_call": l_j}
+            if label.startswith("K0"):
+                t_s, l_s, _, nb_s, _ = find_call(d_m, mlen, d_tape, tw, d_str, slen, paths, [_lib.FIND_KIND_STRING] * k)
+                row.update({"string_ms": round(t_s * 1e3, 3), "string_launches_per_call": l_s, "string_bytes_out": nb_s})
+            min_bytes = covered * 8 + nb + 18 * R * k + 8 * (R + 1) * k
+            row.update({"marshal_ms": round(t_m * 1e3, 3), "marshal_launches_per_call": l_m, "marshal_bytes_out": n_m,
+                        "min_bytes": int(min_bytes), "min_gbs": round(min_bytes / t_j / 1e9, 1),
+                        "frac_of_3.35TBs": round(min_bytes / t_j / 3.35e12, 4),
+                        "timer": "CUDA events around %d back-to-back calls after %d warm-up calls" % (args.calls, args.warmup),
+                        "card": name, "power_limit_w": plimit})
+            print(json.dumps(row), flush=True)
+
+    # K0 batch: the message generated above
+    json_rows("K0 gen_ndjson: %d parking-citations-shaped records, ParseND, copy_strings" % n_rec, d_msg, n, flags,
+              [[[b"Fine"]], [[b"Make"]]])
+    # twitter statuses as NDJSON
+    tw_doc = json.loads(load_fixture("twitter"))
+    block = b"\n".join(json.dumps(x, ensure_ascii=False, separators=(",", ":")).encode() for x in tw_doc["statuses"])
+    nd = b"\n".join([block] * ((args.mib << 20) // (len(block) + 1)))
+    d_nd = torch.full((len(nd) + (1 << 16),), 0x20, dtype=torch.uint8, device=dev)
+    d_nd[:len(nd)] = torch.frombuffer(bytearray(nd), dtype=torch.uint8).to(dev)
+    json_rows("twitter statuses NDJSON, ParseND, copy_strings", d_nd, len(nd), flags,
+              [[[b"user"]], [[b"entities"]], [[b"user"], [b"entities"]]])
+    del d_nd
+    # one cell of about --mib
+    tw = load_fixture("twitter").strip()
+    one = b'{"a":[' + b",".join([tw] * ((args.mib << 20) // (len(tw) + 1))) + b"]}"
+    d_one = torch.full((len(one) + (1 << 16),), 0x20, dtype=torch.uint8, device=dev)
+    d_one[:len(one)] = torch.frombuffer(bytearray(one), dtype=torch.uint8).to(dev)
+    json_rows("{\"a\": [twitter.json x K]}, Parse, copy_strings", d_one, len(one), _lib.FLAG_COPY_STRINGS, [[[b"a"]]])
     ctx.close()
 
 
