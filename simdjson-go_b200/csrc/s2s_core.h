@@ -16,7 +16,7 @@
 //   * the grammar (stage2...go:176-425) is checked per structural against the PREVIOUS structural only: strings are
 //     refined into "follows '{' or ','" (a key in an object) and "follows anything else", so the transition depends
 //     on one predecessor; what depends on the enclosing container is collected as a 3-bit mask {root, object, array}
-//     ANDed per bracket-to-bracket segment and resolved once per bracket after the scope matching (K2d).
+//     ANDed per bracket-to-bracket segment and resolved once per bracket after the scope matching (K2t).
 //
 // This header is portable C++: under nvcc the functions are __host__ __device__, and tests/emu/s2s_emu.cpp compiles
 // the very same templates with a 32-fiber "warp" to check them against the oracle on a machine without a GPU.
@@ -136,10 +136,10 @@ constexpr uint32_t S2S_SSTAGE_BYTES = S2S_STEP_BYTES + 32;           // compacte
 // phase inside its 32-byte sector) fit is staged here and copied out in whole sectors; a denser one stores directly.
 constexpr uint32_t S2S_TSTAGE_WORDS = 640;
 // lists of a staged step's brackets and record starts, kept in the string staging area once Strings.B is out; a step
-// with more of them leaves all its links to K2e / K2f
+// with more of them leaves all its links to K2t
 constexpr uint32_t S2S_LINK_BRK_CAP = 384, S2S_LINK_REC_CAP = 128;
 constexpr uint32_t S2S_LINK_SCAN = 64;  // brackets a close looks back for its partner inside the step
-// brk_kind bit: K2r has written both cross-links of this close (its partner lies in the same step), K2e skips them
+// brk_kind bit: K2r has written both cross-links of this close (its partner lies in the same step), K2t skips them
 constexpr uint8_t BRK_LINKED = 0x80;
 
 // per-slab aggregate (K2p) / exclusive prefix (K2q).  `trail`: string-buffer bytes behind the last real quote of

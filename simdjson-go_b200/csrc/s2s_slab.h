@@ -859,7 +859,7 @@ SJ_HD void s2s_slab(W& wp, const S2sParams& p, uint32_t slab, const S2sWarpMem& 
         const uint32_t sslot = slot0 - ph;               // slot of staging word 0 (modulo 2^32: it may lie in front of slot 0)
         const bool staged = ph + w_step <= S2S_TSTAGE_WORDS;  // warp-uniform, as are the two below
         // brackets and record starts of a staged step are listed in the string staging area, so that the pairs with both
-        // ends in the step are linked here (K2e and K2f then skip them)
+        // ends in the step are linked here (K2t then skips them)
         const bool link_b = staged && b_step != 0 && b_step <= S2S_LINK_BRK_CAP;
         const bool link_r = staged && r_step >= 2 && r_step <= S2S_LINK_REC_CAP && p.rootlink != nullptr;
         uint32_t* const lst = reinterpret_cast<uint32_t*>(sm.sstage);  // [0, BRK_CAP): brackets, then record starts
@@ -896,7 +896,7 @@ SJ_HD void s2s_slab(W& wp, const S2sParams& p, uint32_t slab, const S2sWarpMem& 
             // ---- the grammar, bit-parallel (stage2...go:176-425 as restated by transition_ok): PRE_x = the events whose
             // previous event is of class x; an event is fine inside an object / an array / at the top level iff its
             // (previous class, own class) pair is in the respective set.  What depends on the container is decided
-            // per bracket-to-bracket segment by K2e. ----
+            // per bracket-to-bracket segment by K2t. ----
             const uint64_t O1 = m.open & m.curly & ~qm, O2 = m.open & ~m.curly & ~qm;
             const uint64_t C1 = m.close & m.curly & ~qm, C2 = m.close & ~m.curly & ~qm;
             const uint64_t COMMA = m.comma & ~qm, COLON = m.cc & ~m.comma & ~qm;
@@ -978,7 +978,7 @@ SJ_HD void s2s_slab(W& wp, const S2sParams& p, uint32_t slab, const S2sWarpMem& 
                                 lst[kb - run.brk] = (slot - sslot) | (kind << 10) | ((uint32_t)(dep - run.depth + 4096) << 13);
                             else
                                 p.brk_kind[kb] = (uint8_t)kind;
-                            put(slot, (uint64_t)((opening ? 0x5bu : 0x5du) | (curly ? 0x20u : 0u)) << 56);  // payload: cross-linked below or by K2e
+                            put(slot, (uint64_t)((opening ? 0x5bu : 0x5du) | (curly ? 0x20u : 0u)) << 56);  // payload: cross-linked below or by K2t
                             const uint32_t seg = upto & ~prevm;
                             const uint32_t bad = segbad | ((bdr & seg) ? 1u : 0u) | ((bdo & seg) ? 2u : 0u) | ((bda & seg) ? 4u : 0u);
                             if (bad) wp.atomic_and(p.segmask + (kb >> 2), ~(bad << (8 * (kb & 3))));
@@ -1046,7 +1046,7 @@ SJ_HD void s2s_slab(W& wp, const S2sParams& p, uint32_t slab, const S2sWarpMem& 
             if (link_b || link_r) {
                 const uint64_t tb = s2s_tape_base(p);
                 // a close whose partner -- the nearest bracket in front of it with a smaller depth in front, K2d's rule;
-                // none for a close at the top level -- lies in the step gets both cross-links (K2e's words) and BRK_LINKED
+                // none for a close at the top level -- lies in the step gets both cross-links (K2t's words) and BRK_LINKED
                 for (uint32_t i = lane; link_b && i < b_step; i += 32) {
                     const uint32_t e = lst[i], kind = (e >> 10) & 7u, t = e >> 13;
                     uint32_t linked = 0;

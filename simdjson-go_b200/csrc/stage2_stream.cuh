@@ -10,9 +10,9 @@
 //                      root words of the pairs inside one step, bracket records for the scope matching, number list,
 //                      per-segment grammar masks
 //   K2h s2s_numbers    parse_number (parse_number.go:65) over the number list, one number per thread
-//   K2d s2_min32 + s2_ansv (stage2_common.cuh)    scope matching on the brackets
-//   K2e s2s_link       per bracket: cross-links of { } [ ] (stage2...go:327-334) and the grammar verdict of the segment
-//                      in front of it against the container it lies in; the same launch writes the root words (K2f)
+//   K2t s2t_min + s2t_link (s2s_tile.h)   scope matching on the brackets, tile by tile; per bracket the cross-links of
+//                      { } [ ] (stage2...go:327-334) and the grammar verdict of the segment in front of it against the
+//                      container it lies in; the same launch writes the root words (K2f)
 //
 // The unifiedMachine of the reference (stage2_build_tape_amd64.go:160-446) walks one structural at a time; the
 // per-structural kernels of stage2.cuh gave every structural a thread and spent ~460 warp-instructions per 32
@@ -22,6 +22,7 @@
 #include "common.cuh"
 #include "number.h"
 #include "s2s_slab.h"
+#include "s2s_tile.h"
 #include "stage1.cuh"
 #include "stage2_common.cuh"
 
@@ -90,55 +91,61 @@ __global__ void __launch_bounds__(S2_THREADS) s2s_numbers_kernel(const uint8_t* 
 }
 
 // ---------------------------------------------------------------------------------
-// K2e: per bracket k (and k = nb for the segment behind the last bracket): is every structural of segment k -- the
-// ones behind bracket k-1 up to and including bracket k -- allowed inside the container that is open there?  That
-// container is the scope open right after bracket k-1: the bracket itself if it opens, else the parent of the scope
-// it closes (par = nearest previous bracket with a smaller depth in front of it, K2d).  Closing brackets cross-link
-// the tape words of their pair (stage2...go:327-334), except those K2r has linked already (BRK_LINKED: both ends in
-// one staged step).
+// K2t (s2s_tile.h): K2t-min builds the min hierarchy over the brackets' depths, one CTA per tile; K2t-link then gives
+// every bracket of its tile its par, checks the tile's segments, writes the cross-links and, with the same grid, the
+// root words of records lo .. lo + S2T_TILE - 1
 // ---------------------------------------------------------------------------------
-// The same launch writes the root words (K2f, stage2...go:170,207-218,428-441): record r opens at rootpos[r], its close
-// sits right in front of the next record's open (or is the last word of the tape).  Records whose bit in rootlink K2r
-// has cleared are written already.
-__global__ void __launch_bounds__(S2_THREADS) s2s_link_kernel(const S2sParams p, const int32_t* par, uint32_t nb, uint64_t n_records,
-                                                              uint64_t tape_len) {
-    const uint32_t k = blockIdx.x * S2_THREADS + threadIdx.x;
+constexpr int S2T_THREADS = 1024;
+
+__device__ __forceinline__ int32_t warp_min(int32_t v) {
+#pragma unroll
+    for (int d = 16; d > 0; d >>= 1) v = min(v, __shfl_xor_sync(FULL, v, d));
+    return v;
+}
+
+__global__ void __launch_bounds__(S2T_THREADS) s2t_min_kernel(const int32_t* depth, uint32_t nb, const __grid_constant__ S2tLevels L) {
+    __shared__ int32_t m1[S2T_TILE / 32], m2[S2T_TILE / 1024];
+    const uint32_t lo = blockIdx.x * S2T_TILE, lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+    for (uint32_t i = threadIdx.x; i < S2T_TILE; i += S2T_THREADS) {
+        const int32_t v = warp_min(lo + i < nb ? depth[lo + i] : INT32_MAX);
+        if (lane == 0) m1[i >> 5] = v;
+    }
+    __syncthreads();
+    if (warp < S2T_TILE / 1024) {
+        const uint32_t i = warp * 32 + lane;
+        const int32_t v = m1[i];
+        if (L.nlevels > 1 && (lo >> 5) + i < L.n[1]) L.lv[1][(lo >> 5) + i] = s2t_key(v);
+        const int32_t w = warp_min(v);
+        if (lane == 0) {
+            if (L.nlevels > 2 && (lo >> 10) + warp < L.n[2]) L.lv[2][(lo >> 10) + warp] = s2t_key(w);
+            m2[warp] = w;
+        }
+    }
+    __syncthreads();
+    if (threadIdx.x == 0 && L.nlevels > 3) {
+        int32_t v = m2[0];
+        for (uint32_t q = 1; q < S2T_TILE / 1024; q++) v = min(v, m2[q]);
+        for (int l = 3; l < L.nlevels; l++) atomicMin(L.lv[l] + (lo >> (5 * l)), s2t_key(v));
+    }
+}
+
+__global__ void __launch_bounds__(S2T_THREADS) s2t_link_kernel(const S2sParams p, const __grid_constant__ S2tLevels L, uint32_t nb,
+                                                               uint64_t n_records, uint64_t tape_len) {
+    __shared__ int32_t d_s[S2T_TILE], par_s[S2T_TILE];
+    __shared__ uint8_t k_s[S2T_TILE];
+    const uint32_t lo = blockIdx.x * S2T_TILE;
+    for (uint32_t i = threadIdx.x; i < S2T_TILE && lo + i < nb; i += S2T_THREADS) {
+        d_s[i] = p.brk_depth[lo + i];
+        k_s[i] = p.brk_kind[lo + i];
+    }
+    __syncthreads();
+    const S2tTile v{p.brk_depth, p.brk_kind, d_s, k_s, par_s, lo, &L};
+    for (uint32_t i = threadIdx.x; i < S2T_TILE && lo + i < nb; i += S2T_THREADS) par_s[i] = s2t_par(v, lo + i);
+    __syncthreads();
     const uint64_t tape_base = s2s_tape_base(p);
-    if (k <= n_records && ((p.rootlink[k >> 5] >> (k & 31)) & 1u)) {
-        const uint64_t R = (uint64_t)'r' << 56;
-        const uint64_t open = k == 0 ? 0 : p.rootpos[k];
-        const uint64_t next_open = k == n_records ? tape_len : p.rootpos[k + 1];
-        if (next_open <= tape_len && next_open != 0) {
-            p.tape[open] = R | (tape_base + next_open);
-            p.tape[next_open - 1] = R | (tape_base + open);
-        }
-    }
-    if (k > nb) return;
-    uint32_t ctx = CTX_ROOT;
-    if (k > 0) {
-        const uint32_t kd = p.brk_kind[k - 1] & ~BRK_LINKED;
-        int32_t enc;
-        if (kd == T_OBJ_OPEN || kd == T_ARR_OPEN) {
-            enc = (int32_t)k - 1;
-        } else {
-            const int32_t m = par[k - 1];
-            enc = m >= 0 ? par[m] : -1;
-        }
-        ctx = enc >= 0 ? ((p.brk_kind[enc] & ~BRK_LINKED) == T_OBJ_OPEN ? CTX_OBJ : CTX_ARR) : CTX_ROOT;
-    }
-    const uint32_t sg = (p.segmask[k >> 2] >> (8 * (k & 3))) & 0xffu;
-    if (!((sg >> ctx) & 1u)) atomicOr(p.error, 1u);
-    if (k < nb) {
-        const uint32_t kd = p.brk_kind[k];  // (a linked close carries BRK_LINKED and matches neither kind)
-        if (kd == T_OBJ_CLOSE || kd == T_ARR_CLOSE) {
-            const int32_t m = par[k];
-            if (m >= 0) {
-                const uint32_t otp = p.brk_tp[m], ctp = p.brk_tp[k];
-                p.tape[otp] = ((uint64_t)(kd == T_OBJ_CLOSE ? '{' : '[') << 56) | (tape_base + ctp + 1);
-                p.tape[ctp] = ((uint64_t)(kd == T_OBJ_CLOSE ? '}' : ']') << 56) | (tape_base + otp);
-            }
-        }
-    }
+    for (uint32_t i = threadIdx.x; i < S2T_TILE && lo + i <= nb; i += S2T_THREADS)
+        if (!s2t_segment(p, v, nb, lo + i, tape_base)) atomicOr(p.error, 1u);
+    for (uint32_t i = threadIdx.x; i < S2T_TILE && lo + i <= n_records; i += S2T_THREADS) s2t_root(p, lo + i, n_records, tape_len, tape_base);
 }
 
 }  // namespace sj
