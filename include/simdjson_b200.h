@@ -200,6 +200,12 @@ int sj_parse_count_where(sj_ctx* ctx, const uint8_t* msg, size_t len, uint32_t f
  *   SJ_FIND_KIND_JSON     Element.Iter.MarshalJSON (:394-556): the element as compact JSON text, byte for byte what the
  *                         reference writes (strings escaped like escapeBytes, floats like appendFloat); a scalar gives
  *                         its own text ("abc", 12, true).  Its number is 7: 6 stays an unknown kind (SJ_ERR_ARGUMENT).
+ *   SJ_FIND_KIND_STRING_CVT  Iter.StringCvt (:775-799): strings raw (not escaped), int64 / uint64 in decimal, true /
+ *                         false / null as written, floats as appendFloat (an INF or NaN is SJ_FIND_CONVERT)
+ *   list kinds (sj_find_lists_device / sj_parse_find_lists only): Iter.Array (:1022-1039), then
+ *   SJ_FIND_KIND_ARRAY_FLOAT64  Array.AsFloat (parsed_array.go:145-181)  SJ_FIND_KIND_ARRAY_INT64  Array.AsInteger (:185-232)
+ *   SJ_FIND_KIND_ARRAY_UINT64   Array.AsUint64 (:236-283)     SJ_FIND_KIND_ARRAY_STRING Array.AsString (:287-314)
+ *   SJ_FIND_KIND_ARRAY_STRING_CVT  Array.AsStringCvt (:319-344): each element as SJ_FIND_KIND_STRING_CVT
  * So the first member with the key decides, keys compare on their unescaped bytes, arrays are never entered, and a
  * root or intermediate value that is not an object is SJ_FIND_NOT_OBJECT, not SJ_FIND_NOT_FOUND.  Where amd64 Go and
  * CUDA's conversions differ the cell follows Go: Int() of a float of exactly 2^63 is math.MinInt64 (CVTTSD2SQ), Uint()
@@ -219,8 +225,27 @@ int sj_parse_count_where(sj_ctx* ctx, const uint8_t* msg, size_t len, uint32_t f
  * STRING and JSON path s (counting those paths only, in path order) has str_offsets[s * (row_cap + 1) + r], r = 0 ..
  * rows, into str_bytes, so row r's bytes are [off[r], off[r + 1]) (with no rows, the one entry 0 is written when
  * str_offsets is given).  A call without JSON paths writes what it wrote before they existed.
+ * A list cell is SJ_FIND_OK when the element is an array and the accessor returns no error; its value is the element
+ * count (a STRING_CVT cell's is the byte length).  SJ_FIND_CONVERT: a fresh Element, "next item is not array", "unable
+ * to convert type", an overflow / underflow / negative value, "element in array is not string", StringCvt's "cannot
+ * convert type" and appendFloat's INF / NaN.  SJ_FIND_CORRUPT: "extended beyond tape", "no more values", AdvanceIter's
+ * errors, a string range outside its buffer and any index out of range.  The first failing element decides, and a cell
+ * that is not OK has no elements and no bytes.  The port is literal: AsFloat / AsInteger / AsUint64 read tag words at
+ * even offsets from the word after '[', so a nop or a nested '[' / '{' there is SJ_FIND_CONVERT and a read past the
+ * array's tape is SJ_FIND_CORRUPT; AsString / AsStringCvt step with AdvanceIter, so nops are skipped (a skip of 0 is
+ * SJ_FIND_CORRUPT), a nested scope is stepped over by its link and then rejected, and the first TypeNone tag (']', or any
+ * unknown tag) ends the list as OK.  AsInteger of a float of exactly 2^63 is math.MinInt64; AsUint64 rejects floats
+ * above 2^63 (Iter.Uint accepts them up to 2^64) and makes exactly 2^63 (and NaN) 1<<63.  The work is spread over the
+ * array words, not over cells; only a cell whose AdvanceIter walk meets a nop word (foreign or Deserialize'd tapes) is
+ * finished by one thread, from that word on.
+ * List layout (sj_find_lists_out): list path l (counting list paths only, in path order) has offsets[l * (row_cap + 1)
+ * + r], r = 0 .. rows, into one pool `elems` shared by all list paths in path then row order, so row r's elements are
+ * elems[off[r] .. off[r + 1]): int64 / uint64 / float64 bits, and for ARRAY_STRING / ARRAY_STRING_CVT each element's
+ * byte length.  STRING_CVT, ARRAY_STRING and ARRAY_STRING_CVT paths are variable-length byte columns like STRING and
+ * JSON paths (numbered with them, in path order); a string list row's bytes are its elements back to back, element k
+ * starting at the row's str_offsets entry plus the lengths of elements 0 .. k-1.
  * Limits: 1 to 64 paths, 0 to 32 segments each, 16 KiB of segment bytes in all; else SJ_ERR_ARGUMENT.  A tape longer
- * than 2^32 - 1 words returns SJ_ERR_TOO_LARGE, and so does a JSON path whose cells cover more than SJ_MAX_MARSHAL_TAPE
+ * than 2^32 - 1 words returns SJ_ERR_TOO_LARGE, and so does a JSON or list path whose cells cover more than SJ_MAX_MARSHAL_TAPE
  * tape words in all (only a malformed tape's cells can overlap, so on any other tape this is within the tape).  *rows and *str_bytes are exact even on SJ_ERR_CAPACITY (rows > row_cap
  * or str_bytes > str_cap), when nothing is written; out may be NULL to ask for the sizes.
  * sj_find_device: message, tape, strings and out in device memory, with their lengths (every read stays inside them).
@@ -229,6 +254,10 @@ int sj_parse_count_where(sj_ctx* ctx, const uint8_t* msg, size_t len, uint32_t f
  * tape they are found on the device: the 'r' words that point forward and are not the value word of a string or number (read from word 0),
  * which on every tape the parser or sj_deserialize_device writes are the roots ForEach visits.  sj_parse_find: HOST message in, parse and find on the device, only the columns are copied to `out`
  * (host memory); parse errors return the parse codes.
+ * sj_find_device / sj_parse_find accept every kind but the list kinds (8-12), which return SJ_ERR_ARGUMENT there.
+ * sj_find_lists_device / sj_parse_find_lists take the same arguments plus the list output and *elems (the pool's
+ * element total); *rows, *str_bytes and *elems are exact even on SJ_ERR_CAPACITY (elems > elem_cap too), when nothing is
+ * written, and `lists` may be NULL to ask for the sizes.  Without list paths they compute what the two above compute.
  */
 #define SJ_FIND_OK 0
 #define SJ_FIND_NOT_FOUND 1
@@ -242,6 +271,12 @@ int sj_parse_count_where(sj_ctx* ctx, const uint8_t* msg, size_t len, uint32_t f
 #define SJ_FIND_KIND_BOOL 4
 #define SJ_FIND_KIND_STRING 5
 #define SJ_FIND_KIND_JSON 7
+#define SJ_FIND_KIND_ARRAY_FLOAT64 8
+#define SJ_FIND_KIND_ARRAY_INT64 9
+#define SJ_FIND_KIND_ARRAY_UINT64 10
+#define SJ_FIND_KIND_ARRAY_STRING 11
+#define SJ_FIND_KIND_ARRAY_STRING_CVT 12
+#define SJ_FIND_KIND_STRING_CVT 13
 typedef struct {
     const uint8_t* segments;   /* the key segments laid end to end (host memory) */
     const uint32_t* seg_lens;  /* n_segments lengths */
@@ -263,6 +298,17 @@ int sj_find_device(sj_ctx* ctx, const uint8_t* d_msg, size_t msg_len, const uint
                    const sj_find_out* out, size_t* rows, size_t* str_bytes);
 int sj_parse_find(sj_ctx* ctx, const uint8_t* msg, size_t len, uint32_t flags, const sj_find_path* paths, size_t n_paths,
                   const sj_find_out* out, size_t* rows, size_t* str_bytes);
+typedef struct {
+    int64_t* offsets;  /* [list paths][row_cap + 1]: row r's elements are elems[offsets[r] .. offsets[r + 1]) */
+    uint64_t* elems;   /* elem_cap words: int64 / uint64 / float64 bits; for string lists each element's byte length */
+    size_t elem_cap;
+} sj_find_lists_out;
+int sj_find_lists_device(sj_ctx* ctx, const uint8_t* d_msg, size_t msg_len, const uint64_t* d_tape, size_t tape_len,
+                         const uint8_t* d_strings, size_t strings_len, const sj_find_path* paths, size_t n_paths,
+                         const sj_find_out* out, const sj_find_lists_out* lists, size_t* rows, size_t* str_bytes,
+                         size_t* elems);
+int sj_parse_find_lists(sj_ctx* ctx, const uint8_t* msg, size_t len, uint32_t flags, const sj_find_path* paths, size_t n_paths,
+                        const sj_find_out* out, const sj_find_lists_out* lists, size_t* rows, size_t* str_bytes, size_t* elems);
 
 /*
  * MarshalJSON on the device: Iter.MarshalJSON of a fresh pj.Iter() (parsed_json.go:394-556), byte for byte.  Every

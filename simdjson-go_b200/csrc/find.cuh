@@ -14,15 +14,18 @@
 // Rows are the roots in tape order: stage 2's root list for the tape the context just built, else KC1a / KC1b
 // (tape.cuh), as for countWhere.
 //   KF3 fd_walk         one thread per (path, row), path-major, the path's segments staged in shared memory; the cell's
-//       status, tag, head index and converted value into scratch, a STRING cell's length into `slen`, a JSON cell's
-//       tape words into `jlen`
-//   (JSON paths: the passes of find_json.cuh write each JSON cell's text length into `slen`, `val` and its status)
+//       status, tag, head index and converted value into scratch, a STRING or STRING_CVT cell's length into `slen`, a
+//       JSON or list cell's tape words into `jlen`
+//   (JSON paths: the passes of find_json.cuh write each JSON cell's text length into `slen`, `val` and its status;
+//    list paths: those of find_list.cuh write each list cell's element count, byte length and status)
 //   KF4 fd_len_reduce   per-tile sums of `slen` (scan_groups_kernel twice)
-//   KF5 fd_emit         the columns into the caller's buffers: STRING and JSON offsets from the scan and the STRING
-//       bytes (strings longer than FD_SHORT by their whole warp), and the fixed-size columns with the caller's row stride
-//   (JSON paths: find_json.cuh's KJ6 writes the text behind KF5's offsets)
+//   KF5 fd_emit         the columns into the caller's buffers: the variable-length columns' offsets from the scan, the
+//       STRING bytes (strings longer than FD_SHORT by their whole warp) and STRING_CVT text, and the fixed-size columns
+//       with the caller's row stride
+//   (JSON paths: find_json.cuh's KJ6 writes the text behind KF5's offsets; list paths: find_list.cuh's KL6 the elements)
 #pragma once
 #include "common.cuh"
+#include "fmt.h"
 #include "tape.cuh"
 
 namespace sj {
@@ -32,13 +35,23 @@ constexpr uint64_t FD_SHORT = 32;   // longer strings are copied by their whole 
 
 // cell status (SJ_FIND_*) and path kind (SJ_FIND_KIND_*)
 enum : uint32_t { FD_OK = 0, FD_NOT_FOUND = 1, FD_NOT_OBJECT = 2, FD_CONVERT = 3, FD_CORRUPT = 4 };
-enum : uint32_t { FD_ELEMENT = 0, FD_INT64 = 1, FD_UINT64 = 2, FD_FLOAT64 = 3, FD_BOOL = 4, FD_STRING = 5, FD_JSON = 7 };
+enum : uint32_t {
+    FD_ELEMENT = 0, FD_INT64 = 1, FD_UINT64 = 2, FD_FLOAT64 = 3, FD_BOOL = 4, FD_STRING = 5, FD_JSON = 7,
+    FD_ARRAY_FLOAT64 = 8, FD_ARRAY_INT64 = 9, FD_ARRAY_UINT64 = 10, FD_ARRAY_STRING = 11, FD_ARRAY_STRING_CVT = 12,
+    FD_STRING_CVT = 13
+};
+__host__ __device__ __forceinline__ bool fd_list_kind(uint32_t k) { return k >= FD_ARRAY_FLOAT64 && k <= FD_ARRAY_STRING_CVT; }
+// a variable-length byte column: STRING, JSON, STRING_CVT and the string lists
+__host__ __device__ __forceinline__ bool fd_var_kind(uint32_t k) {
+    return k == FD_STRING || k == FD_JSON || k == FD_STRING_CVT || k == FD_ARRAY_STRING || k == FD_ARRAY_STRING_CVT;
+}
 
 struct FdPath {
     uint32_t seg0, nseg;  // its segments: segs[seg0 .. seg0 + nseg)
     uint32_t kind;
-    uint32_t sidx;        // STRING and JSON paths: index among them (their variable-length column)
-    uint32_t jidx;        // JSON paths: index among them
+    uint32_t sidx;        // variable-length paths (fd_var_kind): index among them (their column)
+    uint32_t jidx;        // JSON and list paths: index among them (their cells are word ranges)
+    uint32_t lidx;        // list paths: index among them
 };
 struct FdSeg {
     uint32_t off, len;    // bytes [off, off + len) of the segment bytes
@@ -56,8 +69,9 @@ struct FindParams {
     uint8_t* tag;
     int64_t* idx;
     uint64_t* val;
-    uint64_t* slen;          // STRING and JSON cells: bytes of the string or text (0 unless OK), at sidx * rows + r
-    uint64_t* jlen;          // JSON cells: tape words of the found element (0 unless found), at jidx * rows + r
+    uint64_t* slen;          // variable-length cells: bytes of the string or text (0 unless OK), at sidx * rows + r
+    uint64_t* jlen;          // JSON and list cells: tape words of the found element (0 unless found), at jidx * rows + r
+    uint64_t* ecnt;          // list cells: elements (0 unless OK), at lidx * rows + r
 };
 
 // the Iter fields the walk uses (parsed_json.go:180-195); n = length of its restricted tape
@@ -267,6 +281,21 @@ __device__ __forceinline__ uint64_t fd_cvttsd2sq(double x) {
     return (uint64_t)__double2ll_rz(x);
 }
 
+// StringCvt's text (parsed_json.go:775-799) of a scalar other than a string, from its tag and value word (the value
+// Int / Uint / Float return for 'l' / 'u' / 'd'); W = false: the length only.  A 'd' must be finite.
+template <bool W>
+__device__ __forceinline__ uint32_t fd_cvt_text(uint32_t t, uint64_t pl, uint8_t* o) {
+    const char* lit = t == 't' ? "true" : t == 'f' ? "false" : "null";
+    if (t == 'l') return fmt_i64<W>((int64_t)pl, o);
+    if (t == 'u') return fmt_u64<W>(pl, o);
+    if (t == 'd') return fmt_double<W>(pl, o);
+    const uint32_t n = t == 'f' ? 5 : 4;
+    if (W)
+        for (uint32_t k = 0; k < n; k++) o[k] = (uint8_t)lit[k];
+    return n;
+}
+__device__ __forceinline__ bool fd_finite(uint64_t bits) { return (bits & 0x7ff0000000000000ull) != 0x7ff0000000000000ull; }
+
 // the accessor of `kind` on the found element e: FD_OK with *val (and the string's bytes for STRING), or its error
 __device__ uint32_t fd_convert(const FindParams& p, const FdIt& e, uint32_t kind, uint64_t* val, const uint8_t** s) {
     const uint32_t t = e.t;
@@ -277,12 +306,24 @@ __device__ uint32_t fd_convert(const FindParams& p, const FdIt& e, uint32_t kind
         *val = t == 't';
         return FD_OK;
     }
-    if (kind == FD_STRING) {  // StringBytes, parsed_json.go:741-749
+    if (kind == FD_STRING || (kind == FD_STRING_CVT && t == '"')) {  // StringBytes, parsed_json.go:741-749
         if (t != '"') return FD_CONVERT;
         if (e.off >= e.n) return FD_CORRUPT;
         const uint64_t len = p.t.tape[e.off];
         if (!tape_string(p.t, e.cur, len, s)) return FD_CORRUPT;
         *val = len;
+        return FD_OK;
+    }
+    if (kind == FD_STRING_CVT) {  // StringCvt, parsed_json.go:775-799 (strings above): the text of Int / Uint / Float
+        if (t == 't' || t == 'f' || t == 'n') {
+            *val = fd_cvt_text<false>(t, 0, nullptr);
+            return FD_OK;
+        }
+        if (t != 'd' && t != 'l' && t != 'u') return FD_CONVERT;  // "cannot convert type %s to string"
+        if (e.off >= e.n) return FD_CORRUPT;                       // "... no more values on tape"
+        const uint64_t pl = p.t.tape[e.off];  // Int of 'l', Uint of 'u' and Float of 'd' return it unchanged
+        if (t == 'd' && !fd_finite(pl)) return FD_CONVERT;         // appendFloat: "INF or NaN number found"
+        *val = fd_cvt_text<false>(t, pl, nullptr);
         return FD_OK;
     }
     if (t != 'd' && t != 'l' && t != 'u') return FD_CONVERT;  // "unable to convert type %v to ..."
@@ -358,6 +399,10 @@ __global__ void __launch_bounds__(FD_THREADS) fd_walk_kernel(const FindParams p)
         idx = (int64_t)e.off - 1;
         if (path.kind == FD_JSON) {
             words = e.n - (uint64_t)idx;  // MarshalJSON's scope: the element's restricted tape [head, n)
+        } else if (fd_list_kind(path.kind)) {  // Iter.Array, parsed_json.go:1022-1039: the array's tape [head, cur)
+            if (e.t != '[') st = FD_CONVERT;          // "next item is not array"
+            else if (e.n < e.cur) st = FD_CORRUPT;    // "object extended beyond tape"
+            else words = e.cur - (uint64_t)idx;
         } else {
             st = fd_convert(p, e, path.kind, &val, &s);
             if (st != FD_OK) val = 0;
@@ -367,8 +412,9 @@ __global__ void __launch_bounds__(FD_THREADS) fd_walk_kernel(const FindParams p)
     p.tag[q] = (uint8_t)tag;
     p.idx[q] = idx;
     p.val[q] = val;
-    if (path.kind == FD_STRING || path.kind == FD_JSON) p.slen[(uint64_t)path.sidx * p.roots.n + r] = val;
-    if (path.kind == FD_JSON) p.jlen[(uint64_t)path.jidx * p.roots.n + r] = words;
+    if (fd_var_kind(path.kind)) p.slen[(uint64_t)path.sidx * p.roots.n + r] = val;
+    if (path.kind == FD_JSON || fd_list_kind(path.kind)) p.jlen[(uint64_t)path.jidx * p.roots.n + r] = words;
+    if (fd_list_kind(path.kind)) p.ecnt[(uint64_t)path.lidx * p.roots.n + r] = 0;
 }
 
 // KF4: per-tile sums of slen
@@ -388,8 +434,8 @@ struct FindEmit {
     uint64_t rows, row_cap;
     uint32_t n_paths, n_str;
     uint32_t str_ntiles;
-    uint8_t str_path[64];        // the path of every STRING and JSON path index
-    uint64_t str_json;           // bit s: column s is a JSON path's (its bytes come from KJ6)
+    uint8_t str_path[64];        // the path of every variable-length column
+    uint64_t str_later;          // bit s: column s is a JSON or string list path's (its bytes come from KJ6 / KL6)
     const uint8_t* st;
     const uint8_t* tag;
     const int64_t* idx;
@@ -406,10 +452,26 @@ struct FindEmit {
     uint8_t* o_bytes;
 };
 
+// `copy` bytes from s to d (none when copy is 0): the whole warp calls it, and copies its strings longer than FD_SHORT
+// together, lane by lane
+__device__ __forceinline__ void fd_copy(const uint8_t* s, uint8_t* d, uint64_t copy) {
+    const uint32_t lane = threadIdx.x & 31;
+    if (copy <= FD_SHORT)
+        for (uint64_t b = 0; b < copy; b++) d[b] = s[b];
+    uint32_t m = __ballot_sync(FULL, copy > FD_SHORT);
+    while (m) {
+        const int src = __ffs(m) - 1;
+        m &= m - 1;
+        const uint8_t* ws = reinterpret_cast<const uint8_t*>(__shfl_sync(FULL, reinterpret_cast<unsigned long long>(s), src));
+        uint8_t* wd = reinterpret_cast<uint8_t*>(__shfl_sync(FULL, reinterpret_cast<unsigned long long>(d), src));
+        const uint64_t wl = __shfl_sync(FULL, copy, src);
+        for (uint64_t b = lane; b < wl; b += 32) wd[b] = ws[b];
+    }
+}
+
 // KF5: blocks [0, str_ntiles) write the string offsets and bytes of TAPE_TILE string cells each; the blocks behind
 // them copy TAPE_TILE cells each of the fixed-size columns to the caller's row stride
 __global__ void __launch_bounds__(TAPE_THREADS) fd_emit_kernel(const FindEmit p) {
-    const uint32_t lane = threadIdx.x & 31;
     if (blockIdx.x >= p.str_ntiles) {
         const uint64_t cells = p.rows * p.n_paths;
         for (int j = 0; j < TAPE_ROUNDS; j++) {
@@ -432,29 +494,25 @@ __global__ void __launch_bounds__(TAPE_THREADS) fd_emit_kernel(const FindEmit p)
         const uint64_t off = carry + block_exclusive_scan(MSum{len}, total).v;
         carry += total.v;
         const uint8_t* s = nullptr;
-        uint64_t copy = 0;  // bytes of a STRING cell
+        uint64_t copy = 0;  // bytes of a STRING or STRING_CVT cell's string
+        uint8_t* d = p.o_bytes + off;
         if (k < n) {
             const uint64_t si = k / p.rows, r = k - si * p.rows;
             int64_t* col = p.o_off + si * (p.row_cap + 1);
             col[r] = (int64_t)off;
             if (r + 1 == p.rows) col[p.rows] = (int64_t)(off + len);
-            if (len && !(p.str_json >> si & 1)) {  // an OK cell: its head word is a string whose range was checked by KF3
-                s = tape_string_ptr(p.t, p.t.tape[p.idx[(uint64_t)p.str_path[si] * p.rows + r]]);
-                copy = len;
+            if (len && !(p.str_later >> si & 1)) {  // an OK cell: a string whose range was checked by KF3, or a scalar
+                const uint64_t h = (uint64_t)p.idx[(uint64_t)p.str_path[si] * p.rows + r];
+                const uint64_t w = p.t.tape[h];
+                if ((w >> 56) == '"') {
+                    s = tape_string_ptr(p.t, w);
+                    copy = len;
+                } else {  // STRING_CVT of a scalar: at most 24 bytes
+                    fd_cvt_text<true>((uint32_t)(w >> 56), tape_value_tag((uint32_t)(w >> 56)) ? p.t.tape[h + 1] : 0, d);
+                }
             }
         }
-        uint8_t* d = p.o_bytes + off;
-        if (copy <= FD_SHORT)
-            for (uint64_t b = 0; b < copy; b++) d[b] = s[b];
-        uint32_t m = __ballot_sync(FULL, copy > FD_SHORT);
-        while (m) {
-            const int src = __ffs(m) - 1;
-            m &= m - 1;
-            const uint8_t* ws = reinterpret_cast<const uint8_t*>(__shfl_sync(FULL, reinterpret_cast<unsigned long long>(s), src));
-            uint8_t* wd = reinterpret_cast<uint8_t*>(__shfl_sync(FULL, reinterpret_cast<unsigned long long>(d), src));
-            const uint64_t wl = __shfl_sync(FULL, copy, src);
-            for (uint64_t b = lane; b < wl; b += 32) wd[b] = ws[b];
-        }
+        fd_copy(s, d, copy);
     }
 }
 

@@ -26,6 +26,7 @@
 #include "consume.cuh"
 #include "find.cuh"
 #include "find_json.cuh"
+#include "find_list.cuh"
 #include "marshal.cuh"
 #include "serialize.cuh"
 #include "zstd.cuh"

@@ -12,7 +12,9 @@ import numpy as np
 from . import _lib
 from ._lib import (COMPRESS_BEST, COMPRESS_DEFAULT, COMPRESS_FAST, COMPRESS_NONE, ERR_CAPACITY, ERR_STAGE1, ERR_STAGE2,
                    ERR_UNSUPPORTED, FIND_CONVERT, FIND_CORRUPT, FIND_KIND_BOOL,
-                   FIND_KIND_ELEMENT, FIND_KIND_FLOAT64, FIND_KIND_INT64, FIND_KIND_JSON, FIND_KIND_STRING, FIND_KIND_UINT64,
+                   FIND_KIND_ARRAY_FLOAT64, FIND_KIND_ARRAY_INT64, FIND_KIND_ARRAY_STRING, FIND_KIND_ARRAY_STRING_CVT,
+                   FIND_KIND_ARRAY_UINT64, FIND_KIND_ELEMENT, FIND_KIND_FLOAT64, FIND_KIND_INT64, FIND_KIND_JSON,
+                   FIND_KIND_STRING, FIND_KIND_STRING_CVT, FIND_KIND_UINT64, FIND_LIST_KINDS, FIND_VAR_KINDS,
                    FIND_NOT_FOUND, FIND_NOT_OBJECT, FIND_OK, FLAG_COPY_STRINGS, FLAG_NDJSON, OK, SjError, Stage1Info)
 
 JSONVALUEMASK = 0xFF_FFFF_FFFF_FFFF  # parsed_json.go:26
@@ -132,7 +134,9 @@ class Context:
         FIND_KIND_* of each.  columns[p] is a FindColumn of numpy arrays (status, tag, index, value, offsets, data):
         `value` is int64 / uint64 / float64 by kind (int64 for ELEMENT, BOOL, STRING and JSON, where it is the length); a
         STRING or JSON column's row r is data[offsets[r]:offsets[r + 1]] (JSON: the element's MarshalJSON text).  Only the columns are copied back; on a parse error
-        rows is 0 and columns is None."""
+        rows is 0 and columns is None.  A list kind's column is a ListColumn: row r's elements are
+        elems[list_offsets[r]:list_offsets[r + 1]] (float64 / int64 / uint64; for string lists each element's byte
+        length, with the bytes in data as for STRING).  Without list kinds the call is sj_parse_find."""
         m = _as_u8(msg)
         flags = (FLAG_NDJSON if ndjson else 0) | (FLAG_COPY_STRINGS if copy_strings else 0)
         cpaths, keep = _find_paths(paths, kinds)
@@ -141,51 +145,79 @@ class Context:
         # STRING path, guessed at its size -- else once more at the exact sizes
         row_cap = int(np.count_nonzero(m == 10)) + 1 if ndjson else 1
         str_cap = m.size + 64
-        n_str = sum(k in (FIND_KIND_STRING, FIND_KIND_JSON) for k in kinds)
+        n_str = sum(k in FIND_VAR_KINDS for k in kinds)
+        n_list = sum(k in FIND_LIST_KINDS for k in kinds)
+        nelems, elem_cap = C.c_size_t(0), m.size // 2 + 1
         for _ in range(2):
             cols = (np.empty((len(paths), row_cap), np.uint8), np.empty((len(paths), row_cap), np.uint8),
                     np.empty((len(paths), row_cap), np.int64), np.empty((len(paths), row_cap), np.uint64),
                     np.empty((n_str, row_cap + 1), np.int64), np.empty(max(str_cap, 1), np.uint8))
             out = _lib.FindOut(*(_addr(a) for a in cols), row_cap, str_cap)
-            rc = self.L.sj_parse_find(self.h, _addr(m) if m.size else None, m.size, flags, cpaths, len(paths), C.byref(out),
-                                      C.byref(rows), C.byref(nbytes))
+            if n_list:
+                lcols = (np.empty((n_list, row_cap + 1), np.int64), np.empty(max(elem_cap, 1), np.uint64))
+                lout = _lib.FindListsOut(_addr(lcols[0]), _addr(lcols[1]), elem_cap)
+                rc = self.L.sj_parse_find_lists(self.h, _addr(m) if m.size else None, m.size, flags, cpaths, len(paths),
+                                                C.byref(out), C.byref(lout), C.byref(rows), C.byref(nbytes), C.byref(nelems))
+            else:
+                rc = self.L.sj_parse_find(self.h, _addr(m) if m.size else None, m.size, flags, cpaths, len(paths),
+                                          C.byref(out), C.byref(rows), C.byref(nbytes))
             if rc != ERR_CAPACITY:
                 break
-            row_cap, str_cap = rows.value, nbytes.value
+            row_cap, str_cap, elem_cap = rows.value, nbytes.value, nelems.value
         if rc in (ERR_STAGE1, ERR_STAGE2):
             return rc, 0, None
         if rc != OK:
             raise SjError(rc)
+        if n_list:
+            cols = cols + lcols
         return rc, rows.value, _find_columns(cols, rows.value, kinds, lambda a, dt: a.view(dt))
 
     def find_device(self, tape, strings, message, paths, kinds, out=None):
         """ForEach + FindElement + accessors over a tape already on this context's device (torch tensors as for
         marshal_device).  `out` (optional) is a tuple of tensors (status u8 [P, R], tag u8 [P, R], index i64 [P, R],
-        value i64 [P, R], str_offsets i64 [S, R + 1], str_bytes u8 [B]) for P paths, S of them STRING or JSON, R >= rows;
-        without it they are allocated at the exact sizes.  Returns (rc, rows, columns): columns[p] is a FindColumn of
-        tensor views (value viewed as float64 for FLOAT64 and uint64 for UINT64), or None unless rc is OK.  rc is
-        SJ_ERR_CAPACITY when `out` is too small (rows and the byte total are still exact, in `rows` and nothing written)."""
+        value i64 [P, R], str_offsets i64 [S, R + 1], str_bytes u8 [B]) for P paths, S of them with a byte column
+        (STRING, JSON, STRING_CVT, ARRAY_STRING, ARRAY_STRING_CVT), R >= rows, and with L list paths two more
+        (list_offsets i64 [L, R + 1], elems i64 [E]); without it they are allocated at the exact sizes.  Returns (rc, rows,
+        columns): columns[p] is a FindColumn (a ListColumn for a list kind) of tensor views (value viewed as float64 for
+        FLOAT64 and uint64 for UINT64, elems as float64 / int64 / uint64 by list kind), or None unless rc is OK.  rc is
+        SJ_ERR_CAPACITY when `out` is too small (rows and the byte total are still exact, in `rows` and nothing written).
+        Without list kinds the call is sj_find_device."""
         import torch
         cpaths, keep = _find_paths(paths, kinds)
         sp, sl = _ptr_len(strings)
         mp, ml = _ptr_len(message)
         tp, tl = _ptr_len(tape)
         rows, nbytes = C.c_size_t(0), C.c_size_t(0)
-        n_str = sum(k in (FIND_KIND_STRING, FIND_KIND_JSON) for k in kinds)
+        n_str = sum(k in FIND_VAR_KINDS for k in kinds)
+        n_list = sum(k in FIND_LIST_KINDS for k in kinds)
+        nelems = C.c_size_t(0)
+
+        def call(o, lo):
+            if n_list:
+                return self.L.sj_find_lists_device(self.h, mp, ml, tp, tl, sp, sl, cpaths, len(paths), o, lo, C.byref(rows),
+                                                   C.byref(nbytes), C.byref(nelems))
+            return self.L.sj_find_device(self.h, mp, ml, tp, tl, sp, sl, cpaths, len(paths), o, C.byref(rows), C.byref(nbytes))
         if out is None:
-            rc = self.L.sj_find_device(self.h, mp, ml, tp, tl, sp, sl, cpaths, len(paths), None, C.byref(rows), C.byref(nbytes))
+            rc = call(None, None)
             if rc not in (OK, ERR_CAPACITY):
                 return rc, rows.value, None
             dev, R = tape.device, rows.value
             out = (torch.empty((len(paths), R), dtype=torch.uint8, device=dev), torch.empty((len(paths), R), dtype=torch.uint8, device=dev),
                    torch.empty((len(paths), R), dtype=torch.int64, device=dev), torch.empty((len(paths), R), dtype=torch.int64, device=dev),
                    torch.empty((n_str, R + 1), dtype=torch.int64, device=dev), torch.empty(max(nbytes.value, 1), dtype=torch.uint8, device=dev))
+            if n_list:
+                out += (torch.empty((n_list, R + 1), dtype=torch.int64, device=dev),
+                        torch.empty(max(nelems.value, 1), dtype=torch.int64, device=dev))
         row_cap = out[0].shape[1]
-        for t, shape in zip(out[:5], [(len(paths), row_cap)] * 4 + [(n_str, row_cap + 1)]):
+        shapes = [(len(paths), row_cap)] * 4 + [(n_str, row_cap + 1)] + ([(n_list, row_cap + 1)] if n_list else [])
+        for t, shape in zip(out[:5] + out[6:7], shapes):
             if tuple(t.shape) != shape or not t.is_contiguous():
                 raise ValueError("find_device: out tensors must be contiguous with shapes %s" % shape)
-        o = _lib.FindOut(*(t.data_ptr() for t in out), row_cap, out[5].numel())
-        rc = self.L.sj_find_device(self.h, mp, ml, tp, tl, sp, sl, cpaths, len(paths), C.byref(o), C.byref(rows), C.byref(nbytes))
+        if len(out) != (8 if n_list else 6):
+            raise ValueError("find_device: out needs %d tensors" % (8 if n_list else 6))
+        o = _lib.FindOut(*(t.data_ptr() for t in out[:6]), row_cap, out[5].numel())
+        lo = _lib.FindListsOut(out[6].data_ptr(), out[7].data_ptr(), out[7].numel()) if n_list else None
+        rc = call(C.byref(o), C.byref(lo) if n_list else None)
         if rc != OK:
             return rc, rows.value, None
         return rc, rows.value, _find_columns(out, rows.value, kinds, _torch_view)
@@ -448,7 +480,7 @@ def _ptr_len(t):
 
 
 class FindColumn(tuple):
-    """one path's column: status, tag, index, value per row; offsets / data for STRING and JSON (else None)"""
+    """one path's column: status, tag, index, value per row; offsets / data for the byte columns (else None)"""
     __slots__ = ()
     _fields = ("status", "tag", "index", "value", "offsets", "data")
 
@@ -461,6 +493,27 @@ class FindColumn(tuple):
     value = property(lambda s: s[3])
     offsets = property(lambda s: s[4])
     data = property(lambda s: s[5])
+
+
+class ListColumn(FindColumn):
+    """a list path's column: FindColumn's fields, then list_offsets (row r's elements are
+    elems[list_offsets[r]:list_offsets[r + 1]]) and elems (float64 / int64 / uint64 values, or for string lists each
+    element's byte length, its bytes back to back in data[offsets[r]:offsets[r + 1]])"""
+    __slots__ = ()
+    _fields = FindColumn._fields + ("list_offsets", "elems")
+
+    list_offsets = property(lambda s: s[6])
+    elems = property(lambda s: s[7])
+
+    def strings(self, r):
+        """row r of a string list as a list of bytes (numpy columns)"""
+        lens = np.asarray(self.elems[self.list_offsets[r]:self.list_offsets[r + 1]])
+        at = int(self.offsets[r])
+        out = []
+        for n in lens.tolist():
+            out.append(bytes(np.asarray(self.data[at:at + n])))
+            at += n
+        return out
 
 
 def _find_paths(paths, kinds):
@@ -484,14 +537,22 @@ def _torch_view(a, dt):
 
 
 def _find_columns(out, rows, kinds, view):
-    status, tag, index, value, offs, data = out
-    cols, s = [], 0
+    status, tag, index, value, offs, data = out[:6]
+    cols, s, l = [], 0, 0
     for p, k in enumerate(kinds):
         dt = np.float64 if k == FIND_KIND_FLOAT64 else np.uint64 if k == FIND_KIND_UINT64 else np.int64
         o = d = None
-        if k in (FIND_KIND_STRING, FIND_KIND_JSON):
+        if k in FIND_VAR_KINDS:
             o, d, s = offs[s, :rows + 1], data, s + 1
-        cols.append(FindColumn(status[p, :rows], tag[p, :rows], index[p, :rows], view(value[p, :rows], dt), o, d))
+        c = (status[p, :rows], tag[p, :rows], index[p, :rows], view(value[p, :rows], dt), o, d)
+        if k in FIND_LIST_KINDS:
+            lo = out[6][l, :rows + 1]
+            n = int(lo[rows]) if rows else 0
+            et = {FIND_KIND_ARRAY_FLOAT64: np.float64, FIND_KIND_ARRAY_UINT64: np.uint64}.get(k, np.int64)
+            cols.append(ListColumn(*c, lo, view(out[7][:n], et)))
+            l += 1
+        else:
+            cols.append(FindColumn(*c))
     return cols
 
 

@@ -21,7 +21,7 @@ EXPORTS = [
     "sj_host_free", "sj_trim_space", "sj_bounds", "sj_parse", "sj_parse_device", "sj_gen_ndjson_device", "sj_parse_nd_sharded_count", "sj_parse_nd_sharded_emit", "sj_exchange_create", "sj_exchange_set_gap", "sj_exchange_set_timeout_ms", "sj_exchange_connect", "sj_exchange_connect_ptrs", "sj_exchange_local", "sj_exchange_bases", "sj_exchange_result", "sj_find_structural_indices", "sj_stage1_device",
     "sj_stage1_launch", "sj_ctx_sync", "sj_event_record", "sj_event_elapsed_ms", "sj_kernel_launches",
     "sj_test_block_masks", "sj_test_geometry", "sj_test_finalize", "sj_test_flatten_bits", "sj_test_parse_strings",
-    "sj_test_parse_numbers", "sj_count_where_device", "sj_parse_count_where", "sj_find_device", "sj_parse_find", "sj_marshal_device", "sj_parse_marshal", "sj_serialize_device", "sj_parse_serialize",
+    "sj_test_parse_numbers", "sj_count_where_device", "sj_parse_count_where", "sj_find_device", "sj_parse_find", "sj_find_lists_device", "sj_parse_find_lists", "sj_marshal_device", "sj_parse_marshal", "sj_serialize_device", "sj_parse_serialize",
     "sj_deserialize_device", "sj_test_set_string_hash_bits", "sj_ctx_set_compress_mode", "sj_test_s2_encode", "sj_test_s2_decode", "sj_test_zstd_encode", "sj_test_zstd_decode", "sj_test_stage2_internal", "sj_test_stage1_ctas", "sj_stream_create", "sj_stream_destroy",
     "sj_stream_write", "sj_stream_close_input", "sj_stream_next", "sj_stream_release",
 ]
@@ -30,6 +30,12 @@ STREAM_END, STREAM_EMPTY, STREAM_BUSY = 7, 8, 9
 FIND_OK, FIND_NOT_FOUND, FIND_NOT_OBJECT, FIND_CONVERT, FIND_CORRUPT = range(5)
 FIND_KIND_ELEMENT, FIND_KIND_INT64, FIND_KIND_UINT64, FIND_KIND_FLOAT64, FIND_KIND_BOOL, FIND_KIND_STRING = range(6)
 FIND_KIND_JSON = 7  # (6 is no kind)
+FIND_KIND_ARRAY_FLOAT64, FIND_KIND_ARRAY_INT64, FIND_KIND_ARRAY_UINT64, FIND_KIND_ARRAY_STRING, FIND_KIND_ARRAY_STRING_CVT = range(8, 13)
+FIND_KIND_STRING_CVT = 13
+FIND_LIST_KINDS = (FIND_KIND_ARRAY_FLOAT64, FIND_KIND_ARRAY_INT64, FIND_KIND_ARRAY_UINT64, FIND_KIND_ARRAY_STRING,
+                   FIND_KIND_ARRAY_STRING_CVT)
+# the kinds with a variable-length byte column
+FIND_VAR_KINDS = (FIND_KIND_STRING, FIND_KIND_JSON, FIND_KIND_STRING_CVT, FIND_KIND_ARRAY_STRING, FIND_KIND_ARRAY_STRING_CVT)
 # Serializer.CompressMode (sj_ctx_set_compress_mode)
 COMPRESS_NONE, COMPRESS_FAST, COMPRESS_DEFAULT, COMPRESS_BEST = range(4)
 FIND_MAX_PATHS, FIND_MAX_SEGMENTS, FIND_MAX_SEGMENT_BYTES = 64, 32, 16384
@@ -52,6 +58,10 @@ class FindPath(C.Structure):
 class FindOut(C.Structure):
     _fields_ = [("status", C.c_void_p), ("tag", C.c_void_p), ("index", C.c_void_p), ("value", C.c_void_p),
                 ("str_offsets", C.c_void_p), ("str_bytes", C.c_void_p), ("row_cap", C.c_size_t), ("str_cap", C.c_size_t)]
+
+
+class FindListsOut(C.Structure):
+    _fields_ = [("offsets", C.c_void_p), ("elems", C.c_void_p), ("elem_cap", C.c_size_t)]
 
 
 class Stage1Info(C.Structure):
@@ -154,6 +164,12 @@ def load():
     L.sj_find_device.argtypes = [vp, vp, sz, vp, sz, vp, sz, C.POINTER(FindPath), sz, C.POINTER(FindOut), szp, szp]
     L.sj_parse_find.restype = i32
     L.sj_parse_find.argtypes = [vp, vp, sz, u32, C.POINTER(FindPath), sz, C.POINTER(FindOut), szp, szp]
+    L.sj_find_lists_device.restype = i32
+    L.sj_find_lists_device.argtypes = [vp, vp, sz, vp, sz, vp, sz, C.POINTER(FindPath), sz, C.POINTER(FindOut),
+                                       C.POINTER(FindListsOut), szp, szp, szp]
+    L.sj_parse_find_lists.restype = i32
+    L.sj_parse_find_lists.argtypes = [vp, vp, sz, u32, C.POINTER(FindPath), sz, C.POINTER(FindOut), C.POINTER(FindListsOut),
+                                      szp, szp, szp]
     L.sj_marshal_device.restype = i32
     L.sj_marshal_device.argtypes = [vp, vp, sz, vp, sz, vp, sz, vp, sz, szp]
     L.sj_parse_marshal.restype = i32

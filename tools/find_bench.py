@@ -13,8 +13,14 @@ Then one JSON line per JSON-cell workload (SJ_FIND_KIND_JSON), each beside sj_ma
   one cell          {"a": [twitter.json x K]} at --mib: the one cell of ["a"]
   json_ms / string_ms / marshal_ms, launches per call, and min_bytes (the tape words the cells cover read once, the
   text written, the columns) over json_ms as a fraction of 3.35 TB/s
+Then one JSON line per list workload (list kinds, sj_find_lists_device):
+  one array         {"a": [about 4.5e7 numbers k / 4]} at --mib: ARRAY_FLOAT64 of ["a"], beside sj_marshal_device
+  K0 lists          the K0 batch with "ll": [two floats] and "tags": [two strings] in every record: ["ll"] as
+                    ARRAY_FLOAT64, ["tags"] as ARRAY_STRING, and both, beside ["Make"] as STRING
+  list_ms, launches per call, elements and bytes out, and min_bytes (the array words read once, the elements, bytes
+  and columns written) over list_ms as a fraction of 3.35 TB/s
 The card's name and power limit are read in the same run.
-usage: python tools/find_bench.py [--mib 512] [--calls 10] [--warmup 3]"""
+usage: python tools/find_bench.py [--mib 512] [--calls 10] [--warmup 3] [--lists-only]"""
 import argparse
 import ctypes as C
 import json
@@ -40,6 +46,7 @@ def main():
     ap.add_argument("--mib", type=int, default=512)
     ap.add_argument("--calls", type=int, default=10)
     ap.add_argument("--warmup", type=int, default=3)
+    ap.add_argument("--lists-only", action="store_true", help="only the list workloads")
     args = ap.parse_args()
 
     import numpy as np
@@ -65,6 +72,8 @@ def main():
         return ms.value / 1e3 / calls
 
     pk = load_fixture("parking-citations").strip()
+    if args.lists_only:
+        return list_rows(args, ctx, L, dev, timed, name, plimit, pk)
     lines = pk.split(b"\n")
     keys = [k.encode() for k in json.loads(lines[0])]
     n_rec = (args.mib << 20) // (len(pk) // len(lines) + 1)
@@ -254,6 +263,117 @@ def main():
     d_one = torch.full((len(one) + (1 << 16),), 0x20, dtype=torch.uint8, device=dev)
     d_one[:len(one)] = torch.frombuffer(bytearray(one), dtype=torch.uint8).to(dev)
     json_rows("{\"a\": [twitter.json x K]}, Parse, copy_strings", d_one, len(one), _lib.FLAG_COPY_STRINGS, [[[b"a"]]])
+    ctx.close()
+
+
+def list_rows(args, ctx, L, dev, timed, name, plimit, pk):
+    import numpy as np
+    import torch
+    from simdjson_b200 import _find_paths, _lib
+
+    def to_dev(b):
+        d = torch.full((len(b) + (1 << 16),), 0x20, dtype=torch.uint8, device=dev)
+        d[:len(b)] = torch.frombuffer(bytearray(b), dtype=torch.uint8).to(dev)
+        return d
+
+    def parsed(d_m, mlen, flags_):
+        tl_, sl_ = C.c_size_t(0), C.c_size_t(0)
+        L.sj_bounds(mlen, C.byref(tl_), C.byref(sl_))
+        d_t = torch.empty(tl_.value, dtype=torch.int64, device=dev)
+        d_s = torch.empty(max(sl_.value, 1), dtype=torch.uint8, device=dev)
+        assert L.sj_parse_device(ctx.h, d_m.data_ptr(), mlen, flags_, d_t.data_ptr(), d_t.numel(), C.byref(tl_),
+                                 d_s.data_ptr(), d_s.numel(), C.byref(sl_)) == 0
+        return d_t, tl_.value, d_s, sl_.value
+
+    def call_timed(fn):
+        for _ in range(args.warmup):
+            fn()
+        l0 = ctx.launches()
+        t = timed(fn, args.calls)
+        return t, (ctx.launches() - l0) / args.calls
+
+    def lists_call(d_m, mlen, d_t, tw, d_s, slen, paths, kinds):
+        cp, keep = _find_paths(paths, kinds)
+        rows, nb, ne = C.c_size_t(0), C.c_size_t(0), C.c_size_t(0)
+        a = (ctx.h, d_m.data_ptr(), mlen, d_t.data_ptr(), tw, d_s.data_ptr(), slen, cp, len(paths))
+        lists = any(k in _lib.FIND_LIST_KINDS for k in kinds)
+        if lists:
+            assert L.sj_find_lists_device(*a, None, None, C.byref(rows), C.byref(nb), C.byref(ne)) in (0, _lib.ERR_CAPACITY)
+        else:
+            assert L.sj_find_device(*a, None, C.byref(rows), C.byref(nb)) in (0, _lib.ERR_CAPACITY)
+        R, k = rows.value, len(paths)
+        ns, nl = sum(x in _lib.FIND_VAR_KINDS for x in kinds), sum(x in _lib.FIND_LIST_KINDS for x in kinds)
+        o = [torch.empty((k, R), dtype=torch.uint8, device=dev), torch.empty((k, R), dtype=torch.uint8, device=dev),
+             torch.empty((k, R), dtype=torch.int64, device=dev), torch.empty((k, R), dtype=torch.int64, device=dev),
+             torch.empty((ns, R + 1), dtype=torch.int64, device=dev), torch.empty(max(nb.value, 1), dtype=torch.uint8, device=dev),
+             torch.empty((nl, R + 1), dtype=torch.int64, device=dev), torch.empty(max(ne.value, 1), dtype=torch.int64, device=dev)]
+        out = _lib.FindOut(*(t.data_ptr() for t in o[:6]), R, nb.value)
+        lo = _lib.FindListsOut(o[6].data_ptr(), o[7].data_ptr(), ne.value)
+
+        def call():
+            if lists:
+                assert L.sj_find_lists_device(*a, C.byref(out), C.byref(lo), C.byref(rows), C.byref(nb), C.byref(ne)) == 0
+            else:
+                assert L.sj_find_device(*a, C.byref(out), C.byref(rows), C.byref(nb)) == 0
+
+        t, launches = call_timed(call)
+        assert bool((o[0] == 0).all()), "a cell is not OK"
+        covered = 0
+        for p, kind in enumerate(kinds):
+            if kind in _lib.FIND_LIST_KINDS:
+                covered += int(((d_t[o[2][p]] & ((1 << 56) - 1)) - o[2][p]).sum())
+        return t, launches, R, nb.value, ne.value, covered
+
+    def marshal_ms(d_m, mlen, d_t, tw, d_s, slen):
+        n_out = C.c_size_t(0)
+        L.sj_marshal_device(ctx.h, d_m.data_ptr(), mlen, d_t.data_ptr(), tw, d_s.data_ptr(), slen, None, 0, C.byref(n_out))
+        o = torch.empty(n_out.value, dtype=torch.uint8, device=dev)
+        t, _ = call_timed(lambda: L.sj_marshal_device(ctx.h, d_m.data_ptr(), mlen, d_t.data_ptr(), tw, d_s.data_ptr(), slen,
+                                                      o.data_ptr(), o.numel(), C.byref(n_out)))
+        return t
+
+    def row(label, mlen, tw, paths, kinds, res, extra):
+        t, launches, R, nb, ne, covered = res
+        min_bytes = covered * 8 + nb + 8 * ne + 18 * R * len(paths) + 8 * (R + 1) * len(paths)
+        r = {"input": label, "input_bytes": mlen, "tape_words": tw, "paths": [p[0].decode() for p in paths],
+             "kinds": list(kinds), "rows": R, "elements_out": ne, "bytes_out": nb, "covered_words": covered,
+             "list_ms": round(t * 1e3, 3), "launches_per_call": launches, "min_bytes": int(min_bytes),
+             "min_gbs": round(min_bytes / t / 1e9, 1), "frac_of_3.35TBs": round(min_bytes / t / 3.35e12, 4),
+             "timer": "CUDA events around %d back-to-back calls after %d warm-up calls" % (args.calls, args.warmup),
+             "card": name, "power_limit_w": plimit}
+        r.update(extra)
+        print(json.dumps(r), flush=True)
+
+    # one array of --mib
+    rng = np.random.default_rng(2024)
+    x = rng.integers(0, 1 << 26, int((args.mib << 20) / 11.9)) / 4.0
+    one = b'{"a":[' + ",".join(map(repr, x.tolist())).encode() + b"]}"
+    d_one = to_dev(one)
+    d_t, tw, d_s, slen = parsed(d_one, len(one), _lib.FLAG_COPY_STRINGS)
+    res = lists_call(d_one, len(one), d_t, tw, d_s, slen, [[b"a"]], [_lib.FIND_KIND_ARRAY_FLOAT64])
+    row('{"a": [%d numbers]}, Parse, copy_strings' % x.size, len(one), tw, [[b"a"]], [_lib.FIND_KIND_ARRAY_FLOAT64], res,
+        {"marshal_ms": round(marshal_ms(d_one, len(one), d_t, tw, d_s, slen) * 1e3, 3)})
+    del d_one, d_t, d_s
+    torch.cuda.empty_cache()
+
+    # the K0 batch with a short float array and a string list in every record
+    recs = [json.loads(line) for line in pk.split(b"\n")]
+    for i, r in enumerate(recs):
+        r["ll"] = [34.0 + i / 64.0, -118.25 - i / 128.0]
+        r["tags"] = ["k%d" % (i % 7), "zone-%d" % (i % 13)]
+    tpl = b"\n".join(json.dumps(r, separators=(",", ":")).encode() for r in recs)
+    n_rec = (args.mib << 20) // (len(tpl) // len(recs) + 1)
+    d_msg = torch.full(((args.mib << 20) + (4 << 20),), 0x20, dtype=torch.uint8, device=dev)
+    glen = C.c_size_t(0)
+    assert L.sj_gen_ndjson_device(ctx.h, tpl, len(tpl), 0, n_rec, d_msg.data_ptr(), d_msg.numel() - (1 << 16), C.byref(glen)) == 0
+    n = glen.value
+    d_t, tw, d_s, slen = parsed(d_msg, n, _lib.FLAG_NDJSON | _lib.FLAG_COPY_STRINGS)
+    label = "K0 gen_ndjson with ll / tags: %d records, ParseND, copy_strings" % n_rec
+    t_s = lists_call(d_msg, n, d_t, tw, d_s, slen, [[b"Make"]], [_lib.FIND_KIND_STRING])[0]
+    for paths, kinds in (([[b"ll"]], [_lib.FIND_KIND_ARRAY_FLOAT64]), ([[b"tags"]], [_lib.FIND_KIND_ARRAY_STRING]),
+                         ([[b"ll"], [b"tags"]], [_lib.FIND_KIND_ARRAY_FLOAT64, _lib.FIND_KIND_ARRAY_STRING])):
+        res = lists_call(d_msg, n, d_t, tw, d_s, slen, paths, kinds)
+        row(label, n, tw, paths, kinds, res, {"make_string_ms": round(t_s * 1e3, 3)})
     ctx.close()
 
 
