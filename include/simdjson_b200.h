@@ -311,6 +311,55 @@ int sj_parse_find_lists(sj_ctx* ctx, const uint8_t* msg, size_t len, uint32_t fl
                         const sj_find_out* out, const sj_find_lists_out* lists, size_t* rows, size_t* str_bytes, size_t* elems);
 
 /*
+ * Array rows of the find: Array.ForEach over every record's array at a row path, each element one row of the find's
+ * columns.  A record is a root, in the find's order.  Its array is a literal port of ParsedJson.ForEach's element
+ * (parsed_json.go:125-138) handed to FindElement(row_path...) (:833-864) and Element.Iter.Array (:1022-1039); a row
+ * path of 0 segments takes elem.Array directly (root arrays, NDJSON lines that are arrays), the one place where 0
+ * segments is not ErrPathNotFound.  The row path's kind must be SJ_FIND_KIND_ELEMENT; it has the limits of a path.
+ * Record status (u8, the list cells' codes): SJ_FIND_OK an array; SJ_FIND_NOT_FOUND FindElement found nothing;
+ * SJ_FIND_NOT_OBJECT it met a value that is not an object; SJ_FIND_CONVERT "next item is not array" or a fresh Element;
+ * SJ_FIND_CORRUPT a malformed tape.  A record that is not OK has no rows.
+ * Rows: the elements Array.ForEach (parsed_array.go:45-56) hands its callback, in order: Advance (:196-223) from the
+ * word after '[' over the array's tape Tape[:end], until TypeNone, quirks included: a nop skips 1 + its skip words (one
+ * more than AdvanceInto), a scope whose link lies behind it, ']', '}', any unknown tag and the end of the array's tape
+ * end the walk silently (ForEach has no error: the walk never makes a record CORRUPT), and an 'r' is an element.
+ * Cells: each (path, row) cell is the find's cell computed from the element's Iter instead of a root: FindElement(path...)
+ * enters a '{' through Iter.Object with the array's tape as its tape, an 'r' through Root, anything else is
+ * SJ_FIND_NOT_OBJECT and a path of 0 segments SJ_FIND_NOT_FOUND; then the accessor of every kind, list kinds included.
+ * Status, tag, index, value, the byte columns and the list pool follow the find's contract above with rows = elements
+ * (row_cap = out->row_cap); `lists` may be NULL when no path has a list kind.
+ * Layout (sj_find_rows_out): record k's rows are [rec_offsets[k], rec_offsets[k + 1]) (rec_offsets[0] = 0, also with no
+ * records), row_tag / row_index the tag byte and tape index of each row's element head.  *records, *rows, *str_bytes and
+ * *elems are exact even on SJ_ERR_CAPACITY (records > record_cap, rows > row_cap, str_bytes > str_cap or elems >
+ * elem_cap), when nothing is written; out, lists and rows_out may be NULL to ask for the sizes.  The array words of all
+ * records above SJ_MAX_MARSHAL_TAPE return SJ_ERR_TOO_LARGE, as for list paths.
+ * The enumeration runs over the array words, not over records: the heads directly inside each array are proposed as its
+ * elements, and each checks that Advance's successor of the one in front of it is itself; a record that fails a check or
+ * meets a nop is walked by one thread.  Launches: KR1 and 4 for the records' word scan, 8 over the array words (none
+ * without them), KR5 and 4 for the row counts' scan, KR6, KR7 and KR8 (21 with array words), with two read-backs, then
+ * the find's passes over the rows (5 with scalar paths); a foreign tape adds the find's 7 that find its roots.
+ * sj_find_rows_device: as sj_find_device (device memory).  sj_parse_find_rows: as sj_parse_find (HOST message, parse
+ * codes on a parse error, only the columns are copied back, into host memory).
+ */
+typedef struct {
+    uint8_t* rec_status;   /* [record_cap]: the row path's cell per record */
+    int64_t* rec_offsets;  /* [record_cap + 1]: record k's rows are [rec_offsets[k], rec_offsets[k + 1]) */
+    uint8_t* row_tag;      /* [row_cap]: the tag byte of each row's element */
+    int64_t* row_index;    /* [row_cap]: the tape index of each row's element head */
+    size_t record_cap;
+} sj_find_rows_out;
+int sj_find_rows_device(sj_ctx* ctx, const uint8_t* d_msg, size_t msg_len, const uint64_t* d_tape, size_t tape_len,
+                        const uint8_t* d_strings, size_t strings_len, const sj_find_path* row_path, const sj_find_path* paths,
+                        size_t n_paths, const sj_find_out* out, const sj_find_lists_out* lists, const sj_find_rows_out* rows_out,
+                        size_t* records, size_t* rows, size_t* str_bytes, size_t* elems);
+int sj_parse_find_rows(sj_ctx* ctx, const uint8_t* msg, size_t len, uint32_t flags, const sj_find_path* row_path,
+                       const sj_find_path* paths, size_t n_paths, const sj_find_out* out, const sj_find_lists_out* lists,
+                       const sj_find_rows_out* rows_out, size_t* records, size_t* rows, size_t* str_bytes, size_t* elems);
+/* test hook: how many records of this context's last array-rows call failed the propose / verify checks and were
+ * walked by one thread (0 on every tape the parser writes) */
+int sj_test_find_rows_serial(sj_ctx* ctx, uint64_t* records);
+
+/*
  * MarshalJSON on the device: Iter.MarshalJSON of a fresh pj.Iter() (parsed_json.go:394-556), byte for byte.  Every
  * root's value as compact JSON, roots joined by one '\n' (no trailing newline); strings escaped like escapeBytes, floats
  * like appendFloat (shortest round-trip digits; fixed notation for 1e-6 <= |x| < 1e21 and 0, else d.ddde+-N).

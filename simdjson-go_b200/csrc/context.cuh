@@ -77,8 +77,10 @@ struct sj_ctx {
     // tape consumers (tape.cuh and its users), each alive within one call only: the call's arguments (countWhere's
     // needles, the find's paths), the scratch of its passes, the Serializer's string dedup, the root list of a foreign
     // tape and the scan that finds it, the output of an sj_parse_* call before its copy to the host, and the per-word
-    // passes of the find's JSON paths (find_json.cuh)
-    DevBuf args, scratch, sz_tab, tc_roots, tc_scan, staging, fj;
+    // passes of the find's JSON paths (find_json.cuh), and the records and element rows of the find's array rows
+    // (find_rows.cuh)
+    DevBuf args, scratch, sz_tab, tc_roots, tc_scan, staging, fj, fr_rec, fr_row;
+    uint64_t find_rows_serial = 0;  // the last array-rows call: records whose rows one thread walked (test hook)
     uint32_t sz_hash_bits = 0;  // test hook: keep only this many bits of the dedup hash (0 = all)
     // the Serializer's compress mode (SJ_COMPRESS_*) and, within one call, the S2 and zstd codecs' buffers (s2.cuh,
     // zstd.cuh): the uncompressed stream and the encoders' chunk slots; the chunk, frame and block lists and the

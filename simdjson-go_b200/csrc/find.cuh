@@ -59,7 +59,8 @@ struct FdSeg {
 
 struct FindParams {
     TapeView t;
-    TapeRows roots;          // one row per root
+    TapeRows roots;          // one row per root; with element rows (find_rows.cuh) roots.n is their count
+    const uint32_t* erow;    // element rows: (head, array end) of row r at 2r, 2r + 1
     uint32_t n_paths;
     const FdPath* paths;
     const FdSeg* segs;
@@ -244,14 +245,19 @@ __device__ uint32_t fd_find_path(const FindParams& p, uint64_t n, uint64_t off, 
     }
 }
 
-// ForEach's element for the root at slot `root`, then FindElement (parsed_json.go:833-864) with Object (:998-1018)
-// and Root (:804-824)
-__device__ uint32_t fd_find(const FindParams& p, uint64_t root, const FdSeg* seg, const uint8_t* bytes, uint32_t nseg,
-                            FdIt& e, bool* fresh) {
-    FdIt it{p.t.n, root, 0, 0, 0}, cp{0, 0, 0, 0, 0};
+// ForEach's element for the root at slot `root` (parsed_json.go:125-138) into cp; false when AdvanceIter fails (the
+// root word is read: it never "ends")
+__device__ __forceinline__ bool fd_root_elem(const FindParams& p, uint64_t root, FdIt& cp) {
+    FdIt it{p.t.n, root, 0, 0, 0};
     uint32_t typ;
-    if (fd_advance_iter(p, it, cp, &typ) != FD_OK) return FD_CORRUPT;  // (the root word is read: never "ended")
+    if (fd_advance_iter(p, it, cp, &typ) != FD_OK) return false;
     fd_advance_into(p, cp);
+    return true;
+}
+
+// FindElement (parsed_json.go:833-864) from the Iter cp, with Object (:998-1018) and Root (:804-824)
+__device__ __forceinline__ uint32_t fd_find_element(const FindParams& p, FdIt cp, const FdSeg* seg, const uint8_t* bytes,
+                                                    uint32_t nseg, FdIt& e, bool* fresh) {
     if (nseg == 0) return FD_NOT_FOUND;
     for (;;) {
         if (cp.t == '{') {
@@ -272,6 +278,14 @@ __device__ uint32_t fd_find(const FindParams& p, uint64_t root, const FdSeg* seg
         }
         return FD_NOT_OBJECT;  // "type %q found before object was found"
     }
+}
+
+// ForEach's element for the root at slot `root`, then FindElement
+__device__ uint32_t fd_find(const FindParams& p, uint64_t root, const FdSeg* seg, const uint8_t* bytes, uint32_t nseg,
+                            FdIt& e, bool* fresh) {
+    FdIt cp{0, 0, 0, 0, 0};
+    if (!fd_root_elem(p, root, cp)) return FD_CORRUPT;
+    return fd_find_element(p, cp, seg, bytes, nseg, e, fresh);
 }
 
 // int64(x) as amd64 lowers it (CVTTSD2SQ): NaN and anything outside int64 give 0x8000000000000000, where CUDA's
@@ -361,7 +375,9 @@ __device__ uint32_t fd_convert(const FindParams& p, const FdIt& e, uint32_t kind
 }
 
 // KF3: one thread per cell, path-major (neighbouring threads take neighbouring rows of one path).  The block stages
-// the segments of the paths its cells belong to: their descriptors, then their bytes.
+// the segments of the paths its cells belong to: their descriptors, then their bytes.  ELEMS: the rows are array
+// elements (find_rows.cuh), each an Iter that Array.ForEach's Advance left on the element's head, over the array's tape.
+template <bool ELEMS>
 __global__ void __launch_bounds__(FD_THREADS) fd_walk_kernel(const FindParams p) {
     extern __shared__ uint8_t fd_smem[];
     const uint64_t cells = p.roots.n * p.n_paths;
@@ -383,10 +399,17 @@ __global__ void __launch_bounds__(FD_THREADS) fd_walk_kernel(const FindParams p)
     const uint32_t pi = (uint32_t)(q / p.roots.n);
     const uint64_t r = q - (uint64_t)pi * p.roots.n;
     const FdPath path = p.paths[pi];
-    const uint64_t root = tape_root(p.roots, r);
     FdIt e{0, 0, 0, 0, 0};
     bool fresh = false;
-    uint32_t st = fd_find(p, root, sseg + (path.seg0 - s_lo), sbytes, path.nseg, e, &fresh);
+    uint32_t st;
+    if (ELEMS) {
+        const uint64_t h = p.erow[2 * r], w = p.t.tape[h];
+        FdIt cp{p.erow[2 * r + 1], h + 1, 0, w & TAPE_VALUE_MASK, (uint32_t)(w >> 56)};
+        fd_calc_next(cp, false);
+        st = fd_find_element(p, cp, sseg + (path.seg0 - s_lo), sbytes, path.nseg, e, &fresh);
+    } else {
+        st = fd_find(p, tape_root(p.roots, r), sseg + (path.seg0 - s_lo), sbytes, path.nseg, e, &fresh);
+    }
     uint32_t tag = 0;
     int64_t idx = -1;
     uint64_t val = 0;

@@ -1,0 +1,286 @@
+// find_rows.cuh -- the array rows of the device find: for every record (a root, in the find's order), the array at a
+// row path, and each of its elements one row of the find's columns.  A literal port of
+//     elem.FindElement(row_path...) -> Element.Iter.Array    (parsed_json.go:833-864, :1022-1039), or elem.Array for a
+//                                                            row path of 0 segments
+//     Array.ForEach(func(i Iter) { i.FindElement(path...) ... })   (parsed_array.go:45-56, Advance :196-223)
+// tests/find_rows_oracle.py is the same port in Python.
+//
+// A record's array is its tape [head, end), laid end to end with the other records' arrays in find_json.cuh's virtual
+// word space (FjWords, KJ0's scan); the work is spread over those words, not over records, as one array may be nearly
+// the whole tape.  The rows are proposed, then verified:
+//   KR1 fr_record   one thread per record: its status, and its array's head and words (KF3's walk for the row path)
+//   (KJ0 over the records' words, KJ1's segmented head scan over the array words)
+//   KR2 fr_stop     the proposed walk: the heads directly inside each array (depth 1 in KJ1's scan).  The first of them
+//       that ends ForEach there -- a TypeNone tag (']', '}', any unknown tag), a nop, or a scope whose link lies behind
+//       it -- lowers the record's stop to its word with atomicMin; the heads in front of the stop are its candidates
+//   KR3 fr_count    the candidates per tile (count and last word, RAgg), scanned; each record's in-tile prefixes
+//   KR4 fr_verify   every candidate and every stop checks that Advance's successor of the candidate in front of it (a
+//       scalar's off + 1 or + 2, a scope's link) is itself, and the first one that it is the word after '['.  So, by
+//       induction from that word, the candidates are ForEach's elements
+//   KR5 fr_finish   per record: its element count, and the last checks (a stop that is a nop, or no stop: the last
+//       successor reaches the end).  A record that fails any check is walked literally by one thread (fr_walk) here
+//   (the counts' scan: each record's first row)
+//   KR6 fr_emit     each candidate of a verified record writes its row: (head, array end) as two uint32 words
+//   KR7 fr_serial_emit   the rows of a record walked by one thread
+//   (KF3 .. with rows = the elements: fd_walk_kernel<true> enters FindElement from each element's Iter)
+//   KR8 fr_out      the record and row columns into the caller's buffers
+#pragma once
+#include "find.cuh"
+#include "find_json.cuh"
+
+namespace sj {
+
+constexpr uint64_t FR_NO_STOP = ~0ull;
+
+// the (candidates, last candidate's virtual word + 1, 0 for none) of a run of words
+struct RAgg {
+    uint64_t n, last;
+};
+__device__ __forceinline__ RAgg agg_combine(const RAgg& a, const RAgg& b) { return RAgg{a.n + b.n, b.last ? b.last : a.last}; }
+__device__ __forceinline__ RAgg agg_shfl_up(const RAgg& a, int d) {
+    return RAgg{__shfl_up_sync(FULL, a.n, d), __shfl_up_sync(FULL, a.last, d)};
+}
+
+// the last candidate's virtual word + 1 alone (KR4 reads no counts)
+struct RLast {
+    uint64_t v;
+};
+__device__ __forceinline__ RLast agg_combine(const RLast& a, const RLast& b) { return RLast{b.v ? b.v : a.v}; }
+__device__ __forceinline__ RLast agg_shfl_up(const RLast& a, int d) { return RLast{__shfl_up_sync(FULL, a.v, d)}; }
+
+struct FrCells {
+    FjWords m;                // the records' arrays (m.rows = records, m.head = each array's '[')
+    TapeView t;
+    const FjAgg* h_tile_pre;  // KJ1's scan
+    const FjAgg* h_grp_pre;
+    uint64_t* stop;           // [records]: the virtual word ForEach's proposed walk stops on, FR_NO_STOP for none
+    const RAgg* c_tile_pre;   // KR3's scan
+    const RAgg* c_grp_pre;
+    RAgg* c_lo;               // [records]: KR3's in-tile prefix in front of a record's '[' / behind its last word
+    RAgg* c_hi;
+    uint8_t* bad;             // [records]: 1 when a check failed
+    uint8_t* serial;          // [records]: 1 when the record is walked by one thread
+    uint64_t* E;              // [records + 1]: element counts, then their exclusive scan and total
+    uint64_t* base;           // [records]: candidates in front of each record
+    unsigned long long* n_serial;  // the records walked by one thread
+    uint32_t* erow;           // [rows][2]
+};
+
+// Advance's next offset after the element whose head is word i (calcNext(false) from off = i + 1)
+__device__ __forceinline__ uint64_t fr_succ(const TapeView& t, uint64_t i) {
+    const uint64_t w = t.tape[i];
+    const uint32_t tag = (uint32_t)(w >> 56);
+    if (tape_value_tag(tag)) return i + 2;
+    if (fd_scope_tag(tag)) return w & TAPE_VALUE_MASK;
+    return i + 1;
+}
+// Advance at head i ends ForEach: a TypeNone tag, a nop (which Advance skips: the record is walked by one thread), or
+// a scope whose link lies behind its word (addNext < 0)
+__device__ __forceinline__ bool fr_stops(const TapeView& t, uint64_t i) {
+    const uint64_t w = t.tape[i];
+    const uint32_t tag = (uint32_t)(w >> 56);
+    return fd_type(tag) == 0 || (fd_scope_tag(tag) && (w & TAPE_VALUE_MASK) < i + 1);
+}
+
+// KR1: one thread per record.  FindElement(row path) as KF3 (no row path: the element itself), then Iter.Array.
+__global__ void __launch_bounds__(256) fr_record_kernel(const FindParams p, uint32_t row_path, uint8_t* st, int64_t* head,
+                                                        uint64_t* words) {
+    const uint64_t r = (uint64_t)blockIdx.x * 256 + threadIdx.x;
+    if (r >= p.roots.n) return;
+    const FdPath path = p.paths[row_path];
+    FdIt cp{0, 0, 0, 0, 0}, e{0, 0, 0, 0, 0};
+    bool fresh = false;
+    uint32_t s = FD_CORRUPT;
+    if (fd_root_elem(p, tape_root(p.roots, r), cp)) {
+        if (path.nseg == 0) {
+            e = cp;
+            s = FD_OK;
+        } else {
+            s = fd_find_element(p, cp, p.segs + path.seg0, p.seg_bytes, path.nseg, e, &fresh);
+        }
+    }
+    uint64_t h = 0, n = 0;
+    if (s == FD_OK) {
+        if (fresh || e.t != '[') s = FD_CONVERT;  // a fresh Element, or "next item is not array"
+        else if (e.n < e.cur) s = FD_CORRUPT;     // "object extended beyond tape"
+        else if (e.cur > e.off) h = e.off - 1, n = e.cur - h;  // a link at or behind the '[': Tape[:end] ends before
+                                                                 // off, and ForEach's first Advance ends it (no rows)
+    }
+    st[r] = (uint8_t)s;
+    head[r] = (int64_t)h;
+    words[r] = n;
+}
+
+// which of this thread's words are heads directly inside their array (bit j; the '[' is none), with their places
+__device__ __forceinline__ uint32_t fr_heads(const FrCells& c, uint64_t base, FjWord (&x)[TAPE_ROUNDS]) {
+    uint64_t w[TAPE_ROUNDS];
+    const FjAgg a = fj_words_agg(c.m, base, w, x);
+    FjAgg total;
+    FjAgg pre = agg_combine(tile_prefix(c.h_tile_pre, c.h_grp_pre, blockIdx.x), block_exclusive_scan(a, total));
+    uint32_t h = 0;
+#pragma unroll
+    for (int j = 0; j < TAPE_ROUNDS; j++) {
+        if (base + j >= c.m.n) break;
+        if (!x[j].first && hagg_out(pre.h, 1) && pre.h.d1 == 1) h |= 1u << j;
+        pre = agg_combine(pre, fj_word_agg(w[j], x[j].i, x[j].first));
+    }
+    return h;
+}
+
+// KR2: every head that stops its walk lowers the record's stop to its word (stop preset to FR_NO_STOP)
+__global__ void __launch_bounds__(TAPE_THREADS) fr_stop_kernel(const FrCells c) {
+    const uint32_t lane = threadIdx.x & 31;
+    const uint64_t base = (uint64_t)blockIdx.x * TAPE_TILE + (uint64_t)threadIdx.x * TAPE_ROUNDS;
+    FjWord x[TAPE_ROUNDS];
+    const uint32_t h = fr_heads(c, base, x);
+#pragma unroll
+    for (int j = 0; j < TAPE_ROUNDS; j++) {
+        const bool stops = (h >> j & 1) && fr_stops(c.t, x[j].i);
+        const uint64_t r = stops ? x[j].r : FR_NO_STOP;
+        // a lane's word j lies behind the lower lanes' words j: the lowest lane of a record has the warp's minimum
+        const uint32_t g = __match_any_sync(FULL, r);
+        if (stops && !(g & ((1u << lane) - 1)) && base + j < *(volatile uint64_t*)&c.stop[r])
+            atomicMin(reinterpret_cast<unsigned long long*>(&c.stop[r]), (unsigned long long)(base + j));
+    }
+}
+
+// this thread's candidates (bit j: a head directly inside its array in front of the record's stop) and their RAgg
+__device__ __forceinline__ uint32_t fr_cands(const FrCells& c, uint64_t base, const FjWord (&x)[TAPE_ROUNDS], uint32_t h, RAgg* a) {
+    uint32_t k = 0;
+    *a = RAgg{0, 0};
+#pragma unroll
+    for (int j = 0; j < TAPE_ROUNDS; j++)
+        if ((h >> j & 1) && base + j < c.stop[x[j].r]) {
+            k |= 1u << j;
+            *a = agg_combine(*a, RAgg{1, base + j + 1});
+        }
+    return k;
+}
+
+// KR3: the candidates of each tile; c_lo / c_hi of every record: the in-tile prefix in front of its '[' / behind its
+// last word
+__global__ void __launch_bounds__(TAPE_THREADS) fr_count_kernel(const FrCells c, RAgg* tile) {
+    const uint64_t base = (uint64_t)blockIdx.x * TAPE_TILE + (uint64_t)threadIdx.x * TAPE_ROUNDS;
+    FjWord x[TAPE_ROUNDS];
+    const uint32_t h = fr_heads(c, base, x);
+    RAgg a, total;
+    const uint32_t k = fr_cands(c, base, x, h, &a);
+    RAgg pre = block_exclusive_scan(a, total);
+#pragma unroll
+    for (int j = 0; j < TAPE_ROUNDS; j++) {
+        if (base + j >= c.m.n) break;
+        if (x[j].first) c.c_lo[x[j].r] = pre;
+        if (k >> j & 1) pre = agg_combine(pre, RAgg{1, base + j + 1});
+        if (x[j].last) c.c_hi[x[j].r] = pre;
+    }
+    if (threadIdx.x == 0) tile[blockIdx.x] = total;
+}
+
+// KR4: the successor check of every candidate and stop
+__global__ void __launch_bounds__(TAPE_THREADS) fr_verify_kernel(const FrCells c) {
+    const uint64_t base = (uint64_t)blockIdx.x * TAPE_TILE + (uint64_t)threadIdx.x * TAPE_ROUNDS;
+    FjWord x[TAPE_ROUNDS];
+    const uint32_t h = fr_heads(c, base, x);
+    RAgg a;
+    const uint32_t k = fr_cands(c, base, x, h, &a);
+    RLast total;
+    RLast pre = agg_combine(RLast{tile_prefix(c.c_tile_pre, c.c_grp_pre, blockIdx.x).last}, block_exclusive_scan(RLast{a.last}, total));
+#pragma unroll
+    for (int j = 0; j < TAPE_ROUNDS; j++) {
+        if (!(h >> j & 1)) continue;
+        if ((k >> j & 1) || base + j == c.stop[x[j].r]) {
+            const uint64_t lo = x[j].s.lo, a0 = base + j - (x[j].i - lo);  // the record's first virtual word (its '[')
+            if (pre.v > a0 ? fr_succ(c.t, pre.v - 1 - a0 + lo) != x[j].i : x[j].i != lo + 1) c.bad[x[j].r] = 1;
+        }
+        if (k >> j & 1) pre.v = base + j + 1;
+    }
+}
+
+// Array.ForEach (parsed_array.go:45-56) over the array Tape[:hi] whose '[' is word lo, in one thread: its element
+// count; with erow set it also writes each element's row there
+__device__ uint64_t fr_walk(const TapeView& t, uint64_t lo, uint64_t hi, uint32_t* erow) {
+    FindParams p;
+    p.t = t;
+    FdIt it{hi, lo + 1, 0, 0, 0};
+    uint64_t n = 0;
+    while (fd_advance(p, it) != 0) {
+        if (erow) {
+            erow[2 * n] = (uint32_t)(it.off - 1);
+            erow[2 * n + 1] = (uint32_t)hi;
+        }
+        n++;
+    }
+    return n;
+}
+
+// KR5: one thread per record
+__global__ void __launch_bounds__(256) fr_finish_kernel(const FrCells c) {
+    const uint64_t r = (uint64_t)blockIdx.x * 256 + threadIdx.x;
+    if (r >= c.m.rows) return;
+    const uint64_t a = c.m.V[c.m.cell0 + r] - c.m.v0, b = c.m.V[c.m.cell0 + r + 1] - c.m.v0;
+    c.serial[r] = 0;
+    c.base[r] = 0;
+    if (a == b) {  // no array: no rows
+        c.E[r] = 0;
+        return;
+    }
+    const uint64_t lo = (uint64_t)c.m.head[r], hi = lo + (b - a), s = c.stop[r];
+    const RAgg l = agg_combine(tile_prefix(c.c_tile_pre, c.c_grp_pre, a / TAPE_TILE), c.c_lo[r]);
+    const RAgg e = agg_combine(tile_prefix(c.c_tile_pre, c.c_grp_pre, (b - 1) / TAPE_TILE), c.c_hi[r]);
+    uint64_t n = e.n - l.n;
+    bool ok = !c.bad[r];
+    if (s != FR_NO_STOP) ok = ok && (c.t.tape[lo + (s - a)] >> 56) != 'N';
+    else ok = ok && (n ? fr_succ(c.t, e.last - 1 - a + lo) >= hi : lo + 1 >= hi);
+    if (!ok) {
+        c.serial[r] = 1;
+        atomicAdd(c.n_serial, 1ull);
+        n = fr_walk(c.t, lo, hi, nullptr);
+    }
+    c.E[r] = n;
+    c.base[r] = l.n;
+}
+
+// KR6: each candidate of a verified record writes its row at the record's first row + its place among the candidates
+__global__ void __launch_bounds__(TAPE_THREADS) fr_emit_kernel(const FrCells c) {
+    const uint64_t base = (uint64_t)blockIdx.x * TAPE_TILE + (uint64_t)threadIdx.x * TAPE_ROUNDS;
+    FjWord x[TAPE_ROUNDS];
+    const uint32_t h = fr_heads(c, base, x);
+    RAgg a, total;
+    const uint32_t k = fr_cands(c, base, x, h, &a);
+    RAgg pre = agg_combine(tile_prefix(c.c_tile_pre, c.c_grp_pre, blockIdx.x), block_exclusive_scan(a, total));
+#pragma unroll
+    for (int j = 0; j < TAPE_ROUNDS; j++) {
+        if (!(k >> j & 1)) continue;
+        const uint64_t r = x[j].r;
+        if (!c.serial[r]) {
+            const uint64_t q = c.E[r] + (pre.n - c.base[r]);
+            c.erow[2 * q] = (uint32_t)x[j].i;
+            c.erow[2 * q + 1] = (uint32_t)x[j].s.hi;
+        }
+        pre.n++;
+    }
+}
+
+// KR7: one thread per record walked by one thread
+__global__ void __launch_bounds__(256) fr_serial_emit_kernel(const FrCells c) {
+    const uint64_t r = (uint64_t)blockIdx.x * 256 + threadIdx.x;
+    if (r >= c.m.rows || !c.serial[r]) return;
+    const uint64_t a = c.m.V[c.m.cell0 + r] - c.m.v0, b = c.m.V[c.m.cell0 + r + 1] - c.m.v0, lo = (uint64_t)c.m.head[r];
+    fr_walk(c.t, lo, lo + (b - a), c.erow + 2 * c.E[r]);
+}
+
+// KR8: the record columns (status, rows' offsets) and the row columns (tag, head index) into the caller's buffers
+__global__ void __launch_bounds__(256) fr_out_kernel(const uint64_t* tape, const uint8_t* st, const uint64_t* E, const uint32_t* erow,
+                                                     uint64_t records, uint64_t rows, uint8_t* o_st, int64_t* o_off, uint8_t* o_tag,
+                                                     int64_t* o_idx) {
+    const uint64_t k = (uint64_t)blockIdx.x * 256 + threadIdx.x;
+    if (k < records) o_st[k] = st[k];
+    if (k <= records) o_off[k] = (int64_t)E[k];
+    if (k < rows) {
+        const uint64_t h = erow[2 * k];
+        o_tag[k] = (uint8_t)(tape[h] >> 56);
+        o_idx[k] = (int64_t)h;
+    }
+}
+
+}  // namespace sj

@@ -27,6 +27,7 @@
 #include "find.cuh"
 #include "find_json.cuh"
 #include "find_list.cuh"
+#include "find_rows.cuh"
 #include "marshal.cuh"
 #include "serialize.cuh"
 #include "zstd.cuh"
@@ -216,7 +217,7 @@ extern "C" void sj_ctx_destroy(sj_ctx* c) {
     DevBuf* bufs[] = {&c->msg,     &c->idx,      &c->desc,     &c->result, &c->s2a,     &c->s2b,    &c->s2c,
                       &c->tape,    &c->strings,  &c->test_in,  &c->test_out, &c->test_aux, &c->args, &c->scratch,
                       &c->sz_tab,  &c->tc_roots, &c->tc_scan,  &c->staging, &c->fj, &c->s2_raw, &c->s2_slots, &c->s2_list,
-                      &c->s2_out,  &c->zx_seq,   &c->zx_src};
+                      &c->s2_out,  &c->zx_seq,   &c->zx_src,   &c->fr_rec, &c->fr_row};
     for (DevBuf* b : bufs) b->release();
     if (c->host_result) cudaFreeHost(c->host_result);
     free(c->pending);
@@ -572,6 +573,7 @@ extern "C" int sj_test_flatten_bits(sj_ctx* c, const uint64_t* masks, size_t nma
 #include "sj_consume.inl"
 #include "sj_marshal.inl"
 #include "sj_find.inl"
+#include "sj_find_rows.inl"
 #include "sj_s2.inl"
 #include "sj_zstd.inl"
 #include "sj_serialize.inl"

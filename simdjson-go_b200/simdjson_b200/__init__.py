@@ -172,6 +172,105 @@ class Context:
             cols = cols + lcols
         return rc, rows.value, _find_columns(cols, rows.value, kinds, lambda a, dt: a.view(dt))
 
+    def parse_find_rows(self, msg, row_path, paths, kinds, ndjson=True, copy_strings=True):
+        """parseMessage, then Array.ForEach over every record's array at `row_path` (a key path; [] takes a record that
+        is itself an array), each element one row of parse_find's columns (FindElement(path...) from the element's Iter
+        + the accessor of each kind, list kinds included): (rc, records, rows, RowIndex, columns).  RowIndex holds
+        rec_status and rec_offsets per record (record k's rows are rec_offsets[k]:rec_offsets[k + 1]) and row_tag and
+        row_index per row (the element head's tag and tape index).  Only the columns are copied back; on a parse error
+        records and rows are 0 and RowIndex and columns are None."""
+        m = _as_u8(msg)
+        flags = (FLAG_NDJSON if ndjson else 0) | (FLAG_COPY_STRINGS if copy_strings else 0)
+        cpaths, keep = _find_paths(paths, kinds)
+        rpath, rkeep = _find_paths([row_path], [FIND_KIND_ELEMENT])
+        records, rows, nbytes, nelems = C.c_size_t(0), C.c_size_t(0), C.c_size_t(0), C.c_size_t(0)
+        n_str = sum(k in FIND_VAR_KINDS for k in kinds)
+        n_list = sum(k in FIND_LIST_KINDS for k in kinds)
+        # the sizes first (no outputs), then the call at the exact sizes
+        rec_cap = row_cap = str_cap = elem_cap = 0
+        cols = lcols = rcols = None
+        for _ in range(2):
+            cols = (np.empty((len(paths), row_cap), np.uint8), np.empty((len(paths), row_cap), np.uint8),
+                    np.empty((len(paths), row_cap), np.int64), np.empty((len(paths), row_cap), np.uint64),
+                    np.empty((n_str, row_cap + 1), np.int64), np.empty(max(str_cap, 1), np.uint8))
+            out = _lib.FindOut(*(_addr(a) for a in cols), row_cap, str_cap)
+            lcols = (np.empty((max(n_list, 1), row_cap + 1), np.int64), np.empty(max(elem_cap, 1), np.uint64))
+            lout = _lib.FindListsOut(_addr(lcols[0]), _addr(lcols[1]), elem_cap)
+            rcols = (np.empty(max(rec_cap, 1), np.uint8), np.empty(rec_cap + 1, np.int64), np.empty(max(row_cap, 1), np.uint8),
+                     np.empty(max(row_cap, 1), np.int64))
+            rout = _lib.FindRowsOut(*(_addr(a) for a in rcols), rec_cap)
+            rc = self.L.sj_parse_find_rows(self.h, _addr(m) if m.size else None, m.size, flags, rpath, cpaths, len(paths),
+                                           C.byref(out), C.byref(lout), C.byref(rout), C.byref(records), C.byref(rows),
+                                           C.byref(nbytes), C.byref(nelems))
+            if rc != ERR_CAPACITY:
+                break
+            rec_cap, row_cap, str_cap, elem_cap = records.value, rows.value, nbytes.value, nelems.value
+        if rc in (ERR_STAGE1, ERR_STAGE2):
+            return rc, 0, 0, None, None
+        if rc != OK:
+            raise SjError(rc)
+        R, n = records.value, rows.value
+        index = RowIndex(rcols[0][:R], rcols[1][:R + 1], rcols[2][:n], rcols[3][:n])
+        return rc, R, n, index, _find_columns(cols + lcols, n, kinds, lambda a, dt: a.view(dt))
+
+    def find_rows_device(self, tape, strings, message, row_path, paths, kinds, out=None):
+        """Array.ForEach over every record's array at `row_path` on a tape already on this context's device (torch
+        tensors as for find_device): (rc, records, rows, RowIndex, columns) as parse_find_rows, of tensor views.  `out`
+        (optional) is find_device's tuple with L list paths' two tensors always present (list_offsets [L, R + 1], elems
+        [E]), then rec_status u8 [N], rec_offsets i64 [N + 1], row_tag u8 [R], row_index i64 [R]; without it the tensors
+        are allocated at the exact sizes.  rc is SJ_ERR_CAPACITY when `out` is too small (the sizes are still exact)."""
+        import torch
+        cpaths, keep = _find_paths(paths, kinds)
+        rpath, rkeep = _find_paths([row_path], [FIND_KIND_ELEMENT])
+        sp, sl = _ptr_len(strings)
+        mp, ml = _ptr_len(message)
+        tp, tl = _ptr_len(tape)
+        records, rows, nbytes, nelems = C.c_size_t(0), C.c_size_t(0), C.c_size_t(0), C.c_size_t(0)
+        n_str = sum(k in FIND_VAR_KINDS for k in kinds)
+        n_list = sum(k in FIND_LIST_KINDS for k in kinds)
+
+        def call(o, lo, ro):
+            return self.L.sj_find_rows_device(self.h, mp, ml, tp, tl, sp, sl, rpath, cpaths, len(paths), o, lo, ro,
+                                              C.byref(records), C.byref(rows), C.byref(nbytes), C.byref(nelems))
+        if out is None:
+            rc = call(None, None, None)
+            if rc not in (OK, ERR_CAPACITY):
+                return rc, records.value, rows.value, None, None
+            dev, N, R = tape.device, records.value, rows.value
+            u8, i64 = torch.uint8, torch.int64
+            out = (torch.empty((len(paths), R), dtype=u8, device=dev), torch.empty((len(paths), R), dtype=u8, device=dev),
+                   torch.empty((len(paths), R), dtype=i64, device=dev), torch.empty((len(paths), R), dtype=i64, device=dev),
+                   torch.empty((n_str, R + 1), dtype=i64, device=dev), torch.empty(max(nbytes.value, 1), dtype=u8, device=dev),
+                   torch.empty((n_list, R + 1), dtype=i64, device=dev), torch.empty(max(nelems.value, 1), dtype=i64, device=dev),
+                   torch.empty(max(N, 1), dtype=u8, device=dev), torch.empty(N + 1, dtype=i64, device=dev),
+                   torch.empty(max(R, 1), dtype=u8, device=dev), torch.empty(max(R, 1), dtype=i64, device=dev))
+        if len(out) != 12:
+            raise ValueError("find_rows_device: out needs 12 tensors")
+        row_cap = out[0].shape[1]
+        shapes = [(len(paths), row_cap)] * 4 + [(n_str, row_cap + 1), None, (n_list, row_cap + 1)]
+        for t, shape in zip(out, shapes):
+            if (shape is not None and tuple(t.shape) != shape) or not t.is_contiguous():
+                raise ValueError("find_rows_device: out tensors must be contiguous with shapes %s" % shape)
+        rec_cap = out[9].numel() - 1
+        if out[8].numel() < rec_cap or out[10].numel() < row_cap or out[11].numel() < row_cap:
+            raise ValueError("find_rows_device: record and row columns smaller than their caps")
+        o = _lib.FindOut(*(t.data_ptr() for t in out[:6]), row_cap, out[5].numel())
+        lo = _lib.FindListsOut(out[6].data_ptr(), out[7].data_ptr(), out[7].numel())
+        ro = _lib.FindRowsOut(*(t.data_ptr() for t in out[8:12]), rec_cap)
+        rc = call(C.byref(o), C.byref(lo), C.byref(ro))
+        N, R = records.value, rows.value
+        if rc != OK:
+            return rc, N, R, None, None
+        index = RowIndex(out[8][:N], out[9][:N + 1], out[10][:R], out[11][:R])
+        return rc, N, R, index, _find_columns(out, R, kinds, _torch_view)
+
+    def find_rows_serial(self):
+        """test hook: the records of the last array-rows call whose rows one thread walked (sj_test_find_rows_serial)"""
+        n = C.c_uint64(0)
+        if self.L.sj_test_find_rows_serial(self.h, C.byref(n)) != OK:
+            raise SjError(ERR_ARGUMENT)
+        return n.value
+
     def find_device(self, tape, strings, message, paths, kinds, out=None):
         """ForEach + FindElement + accessors over a tape already on this context's device (torch tensors as for
         marshal_device).  `out` (optional) is a tuple of tensors (status u8 [P, R], tag u8 [P, R], index i64 [P, R],
@@ -514,6 +613,21 @@ class ListColumn(FindColumn):
             out.append(bytes(np.asarray(self.data[at:at + n])))
             at += n
         return out
+
+
+class RowIndex(tuple):
+    """the records and rows of a find over array rows: rec_status and rec_offsets per record (record k's rows are
+    rec_offsets[k]:rec_offsets[k + 1]), row_tag and row_index per row (its element head's tag byte and tape index)"""
+    __slots__ = ()
+    _fields = ("rec_status", "rec_offsets", "row_tag", "row_index")
+
+    def __new__(cls, *a):
+        return tuple.__new__(cls, a)
+
+    rec_status = property(lambda s: s[0])
+    rec_offsets = property(lambda s: s[1])
+    row_tag = property(lambda s: s[2])
+    row_index = property(lambda s: s[3])
 
 
 def _find_paths(paths, kinds):

@@ -19,8 +19,20 @@ Then one JSON line per list workload (list kinds, sj_find_lists_device):
                     ARRAY_FLOAT64, ["tags"] as ARRAY_STRING, and both, beside ["Make"] as STRING
   list_ms, launches per call, elements and bytes out, and min_bytes (the array words read once, the elements, bytes
   and columns written) over list_ms as a fraction of 3.35 TB/s
+Then one JSON line per array-rows workload (sj_find_rows_device: every record's array at a row path, one row per
+element):
+  statuses          {"statuses": [twitter's statuses x k]} at --mib, row path ["statuses"]: ["user","screen_name"]
+                    STRING, ["retweet_count"] INT64, ["id"] UINT64, ["entities"] JSON, each alone and all four; beside
+                    sj_marshal_device and ["statuses"] as one JSON cell (sj_find_lists_device) of the same tape
+  github_events     github_events' 30 events repeated into one root array at --mib, row path []: ["type"] STRING,
+                    ["payload"] JSON, each alone and both; beside sj_marshal_device
+  hashtags          twitter's statuses one per line at --mib, row path ["entities","hashtags"]: ["text"] STRING,
+                    ["indices"] ARRAY_INT64, each alone and both; beside sj_marshal_device
+  rows_ms, launches per call, records, rows, bytes and elements out, records walked by one thread, and min_bytes
+  (the array words read once, the record and row columns, the cells, bytes and elements written) over rows_ms as a
+  fraction of 3.35 TB/s
 The card's name and power limit are read in the same run.
-usage: python tools/find_bench.py [--mib 512] [--calls 10] [--warmup 3] [--lists-only]"""
+usage: python tools/find_bench.py [--mib 512] [--calls 10] [--warmup 3] [--lists-only | --rows-only]"""
 import argparse
 import ctypes as C
 import json
@@ -47,6 +59,7 @@ def main():
     ap.add_argument("--calls", type=int, default=10)
     ap.add_argument("--warmup", type=int, default=3)
     ap.add_argument("--lists-only", action="store_true", help="only the list workloads")
+    ap.add_argument("--rows-only", action="store_true", help="only the array-rows workloads")
     args = ap.parse_args()
 
     import numpy as np
@@ -74,6 +87,8 @@ def main():
     pk = load_fixture("parking-citations").strip()
     if args.lists_only:
         return list_rows(args, ctx, L, dev, timed, name, plimit, pk)
+    if args.rows_only:
+        return array_rows(args, ctx, L, dev, timed, name, plimit)
     lines = pk.split(b"\n")
     keys = [k.encode() for k in json.loads(lines[0])]
     n_rec = (args.mib << 20) // (len(pk) // len(lines) + 1)
@@ -266,10 +281,10 @@ def main():
     ctx.close()
 
 
-def list_rows(args, ctx, L, dev, timed, name, plimit, pk):
-    import numpy as np
+def dev_tools(args, ctx, L, dev, timed):
+    """(to_dev, parsed, call_timed, marshal_ms): a message in HBM, its tape, a timed call with its launches, and
+    sj_marshal_device of a tape timed the same way"""
     import torch
-    from simdjson_b200 import _find_paths, _lib
 
     def to_dev(b):
         d = torch.full((len(b) + (1 << 16),), 0x20, dtype=torch.uint8, device=dev)
@@ -291,6 +306,24 @@ def list_rows(args, ctx, L, dev, timed, name, plimit, pk):
         l0 = ctx.launches()
         t = timed(fn, args.calls)
         return t, (ctx.launches() - l0) / args.calls
+
+    def marshal_ms(d_m, mlen, d_t, tw, d_s, slen):
+        n_out = C.c_size_t(0)
+        L.sj_marshal_device(ctx.h, d_m.data_ptr(), mlen, d_t.data_ptr(), tw, d_s.data_ptr(), slen, None, 0, C.byref(n_out))
+        o = torch.empty(n_out.value, dtype=torch.uint8, device=dev)
+        t, _ = call_timed(lambda: L.sj_marshal_device(ctx.h, d_m.data_ptr(), mlen, d_t.data_ptr(), tw, d_s.data_ptr(), slen,
+                                                      o.data_ptr(), o.numel(), C.byref(n_out)))
+        return t
+
+    return to_dev, parsed, call_timed, marshal_ms
+
+
+def list_rows(args, ctx, L, dev, timed, name, plimit, pk):
+    import numpy as np
+    import torch
+    from simdjson_b200 import _find_paths, _lib
+
+    to_dev, parsed, call_timed, marshal_ms = dev_tools(args, ctx, L, dev, timed)
 
     def lists_call(d_m, mlen, d_t, tw, d_s, slen, paths, kinds):
         cp, keep = _find_paths(paths, kinds)
@@ -323,14 +356,6 @@ def list_rows(args, ctx, L, dev, timed, name, plimit, pk):
             if kind in _lib.FIND_LIST_KINDS:
                 covered += int(((d_t[o[2][p]] & ((1 << 56) - 1)) - o[2][p]).sum())
         return t, launches, R, nb.value, ne.value, covered
-
-    def marshal_ms(d_m, mlen, d_t, tw, d_s, slen):
-        n_out = C.c_size_t(0)
-        L.sj_marshal_device(ctx.h, d_m.data_ptr(), mlen, d_t.data_ptr(), tw, d_s.data_ptr(), slen, None, 0, C.byref(n_out))
-        o = torch.empty(n_out.value, dtype=torch.uint8, device=dev)
-        t, _ = call_timed(lambda: L.sj_marshal_device(ctx.h, d_m.data_ptr(), mlen, d_t.data_ptr(), tw, d_s.data_ptr(), slen,
-                                                      o.data_ptr(), o.numel(), C.byref(n_out)))
-        return t
 
     def row(label, mlen, tw, paths, kinds, res, extra):
         t, launches, R, nb, ne, covered = res
@@ -374,6 +399,109 @@ def list_rows(args, ctx, L, dev, timed, name, plimit, pk):
                          ([[b"ll"], [b"tags"]], [_lib.FIND_KIND_ARRAY_FLOAT64, _lib.FIND_KIND_ARRAY_STRING])):
         res = lists_call(d_msg, n, d_t, tw, d_s, slen, paths, kinds)
         row(label, n, tw, paths, kinds, res, {"make_string_ms": round(t_s * 1e3, 3)})
+    ctx.close()
+
+
+def array_rows(args, ctx, L, dev, timed, name, plimit):
+    import torch
+    from simdjson_b200 import _find_paths, _lib
+    from tests.util import load_fixture
+
+    to_dev, parsed, call_timed, marshal_ms = dev_tools(args, ctx, L, dev, timed)
+    i64, u8 = torch.int64, torch.uint8
+
+    def rows_call(d_m, mlen, d_t, tw, d_s, slen, row_path, paths, kinds):
+        cp, keep = _find_paths(paths, kinds)
+        rp, rkeep = _find_paths([row_path], [_lib.FIND_KIND_ELEMENT])
+        n = [C.c_size_t(0) for _ in range(4)]  # records, rows, bytes, elements
+        a = (ctx.h, d_m.data_ptr(), mlen, d_t.data_ptr(), tw, d_s.data_ptr(), slen, rp, cp, len(paths))
+        assert L.sj_find_rows_device(*a, None, None, None, *(C.byref(x) for x in n)) in (0, _lib.ERR_CAPACITY)
+        N, R, nb, ne = (x.value for x in n)
+        k = len(paths)
+        ns, nl = sum(x in _lib.FIND_VAR_KINDS for x in kinds), sum(x in _lib.FIND_LIST_KINDS for x in kinds)
+        o = [torch.empty((k, R), dtype=u8, device=dev), torch.empty((k, R), dtype=u8, device=dev),
+             torch.empty((k, R), dtype=i64, device=dev), torch.empty((k, R), dtype=i64, device=dev),
+             torch.empty((ns, R + 1), dtype=i64, device=dev), torch.empty(max(nb, 1), dtype=u8, device=dev),
+             torch.empty((nl, R + 1), dtype=i64, device=dev), torch.empty(max(ne, 1), dtype=i64, device=dev),
+             torch.empty(max(N, 1), dtype=u8, device=dev), torch.empty(N + 1, dtype=i64, device=dev),
+             torch.empty(max(R, 1), dtype=u8, device=dev), torch.empty(max(R, 1), dtype=i64, device=dev)]
+        out = _lib.FindOut(*(t.data_ptr() for t in o[:6]), R, nb)
+        lo = _lib.FindListsOut(o[6].data_ptr(), o[7].data_ptr(), ne)
+        ro = _lib.FindRowsOut(*(t.data_ptr() for t in o[8:12]), N)
+
+        def call():
+            assert L.sj_find_rows_device(*a, C.byref(out), C.byref(lo), C.byref(ro), *(C.byref(x) for x in n)) == 0
+
+        t, launches = call_timed(call)
+        serial = C.c_uint64(0)
+        L.sj_test_find_rows_serial(ctx.h, C.byref(serial))
+        ok = int((o[8][:N] == 0).sum())  # records with an array
+        # the array words: each record's [head, end), its '[' one word in front of its first row
+        first = o[9][:N][o[9][1:N + 1] > o[9][:N]]
+        heads = o[11][first] - 1
+        covered = int(((d_t[heads] & ((1 << 56) - 1)) - heads).sum())
+        return t, launches, N, R, nb, ne, covered, serial.value, ok
+
+    def line(label, mlen, tw, row_path, paths, kinds, res, extra):
+        t, launches, N, R, nb, ne, covered, serial, ok = res
+        ns = sum(x in _lib.FIND_VAR_KINDS for x in kinds)
+        min_bytes = covered * 8 + 9 * N + 8 + 9 * R + 18 * R * len(paths) + 8 * (R + 1) * ns + nb + 8 * ne
+        r = {"input": label, "input_bytes": mlen, "tape_words": tw, "row_path": [x.decode() for x in row_path],
+             "paths": [".".join(x.decode() for x in p) for p in paths], "kinds": list(kinds), "records": N, "records_ok": ok, "rows": R,
+             "bytes_out": nb, "elements_out": ne, "serial_records": serial, "covered_words": covered,
+             "rows_ms": round(t * 1e3, 3), "launches_per_call": launches, "min_bytes": int(min_bytes),
+             "min_gbs": round(min_bytes / t / 1e9, 1), "frac_of_3.35TBs": round(min_bytes / t / 3.35e12, 4),
+             "timer": "CUDA events around %d back-to-back calls after %d warm-up calls" % (args.calls, args.warmup),
+             "card": name, "power_limit_w": plimit}
+        r.update(extra)
+        print(json.dumps(r), flush=True)
+
+    def one_json_cell_ms(d_m, mlen, d_t, tw, d_s, slen, path):
+        cp, keep = _find_paths([path], [_lib.FIND_KIND_JSON])
+        rows, nb, ne = C.c_size_t(0), C.c_size_t(0), C.c_size_t(0)
+        a = (ctx.h, d_m.data_ptr(), mlen, d_t.data_ptr(), tw, d_s.data_ptr(), slen, cp, 1)
+        assert L.sj_find_lists_device(*a, None, None, C.byref(rows), C.byref(nb), C.byref(ne)) in (0, _lib.ERR_CAPACITY)
+        R = rows.value
+        o = [torch.empty((1, R), dtype=u8, device=dev), torch.empty((1, R), dtype=u8, device=dev),
+             torch.empty((1, R), dtype=i64, device=dev), torch.empty((1, R), dtype=i64, device=dev),
+             torch.empty((1, R + 1), dtype=i64, device=dev), torch.empty(max(nb.value, 1), dtype=u8, device=dev)]
+        out = _lib.FindOut(*(t.data_ptr() for t in o), R, nb.value)
+        t, _ = call_timed(lambda: L.sj_find_lists_device(*a, C.byref(out), None, C.byref(rows), C.byref(nb), C.byref(ne)))
+        assert bool((o[0] == 0).all())
+        return t
+
+    def workload(label, doc, flags, row_path, path_sets, json_cell=None):
+        d_m = to_dev(doc)
+        d_t, tw, d_s, slen = parsed(d_m, len(doc), flags)
+        extra = {"marshal_ms": round(marshal_ms(d_m, len(doc), d_t, tw, d_s, slen) * 1e3, 3)}
+        if json_cell:
+            extra["one_json_cell_ms"] = round(one_json_cell_ms(d_m, len(doc), d_t, tw, d_s, slen, json_cell) * 1e3, 3)
+        for paths, kinds in path_sets:
+            res = rows_call(d_m, len(doc), d_t, tw, d_s, slen, row_path, paths, kinds)
+            line(label, len(doc), tw, row_path, paths, kinds, res, extra)
+        del d_m, d_t, d_s
+        torch.cuda.empty_cache()
+
+    def sets(pk):
+        return [([p], [k]) for p, k in pk] + [([p for p, _ in pk], [k for _, k in pk])]
+
+    size = args.mib << 20
+    tw_doc = json.loads(load_fixture("twitter"))
+    statuses = [json.dumps(x, separators=(",", ":")).encode() for x in tw_doc["statuses"]]
+    body = b",".join(statuses)
+    doc = b'{"statuses":[' + b",".join([body] * max(1, size // (len(body) + 1))) + b"]}"
+    workload("{\"statuses\": [twitter statuses x k]}, Parse, copy_strings", doc, _lib.FLAG_COPY_STRINGS, [b"statuses"],
+             sets([([b"user", b"screen_name"], _lib.FIND_KIND_STRING), ([b"retweet_count"], _lib.FIND_KIND_INT64),
+                   ([b"id"], _lib.FIND_KIND_UINT64), ([b"entities"], _lib.FIND_KIND_JSON)]), json_cell=[b"statuses"])
+    events = load_fixture("github_events").strip()
+    body = events[1:-1].strip()
+    doc = b"[" + b",".join([body] * max(1, size // (len(body) + 1))) + b"]"
+    workload("github_events repeated into one root array, Parse, copy_strings", doc, _lib.FLAG_COPY_STRINGS, [],
+             sets([([b"type"], _lib.FIND_KIND_STRING), ([b"payload"], _lib.FIND_KIND_JSON)]))
+    lines = b"\n".join(statuses)
+    doc = b"\n".join([lines] * max(1, size // (len(lines) + 1)))
+    workload("twitter statuses as NDJSON, ParseND, copy_strings", doc, _lib.FLAG_NDJSON | _lib.FLAG_COPY_STRINGS,
+             [b"entities", b"hashtags"], sets([([b"text"], _lib.FIND_KIND_STRING), ([b"indices"], _lib.FIND_KIND_ARRAY_INT64)]))
     ctx.close()
 
 

@@ -79,6 +79,27 @@ for tape in (own, own.clone()):
     rc, sizes, (t2, s2, m2) = ctx.deserialize_device(stream)
     assert rc == 0 and ctx.marshal_device(t2[:sizes[0]], s2[:sizes[1]], m2[:sizes[2]])[2].cpu().numpy().tobytes() == want_text
     n += 1
+# the find's array rows (find_rows.cuh): KR1 .. KR8 and KF3 from elements, on the context's own tape and on the same
+# tape passed as foreign, with a nop among the elements so that one record takes the one-thread walk
+from tests import find_rows_oracle as fr
+
+rdoc = b'{"a":[{"s":"x","n":[1,2]},3,{"s":"yz"},[1]]}\n{"a":[]}\n{"b":1}\n[{"s":"q"},true]'
+rc_o, tape_r, str_r, (off_r, len_r) = o.parse(rdoc, ndjson=True)
+rpaths, rkinds = [[b"s"], [b"n"], [b"s"]], [fo.STRING, 9, 7]
+for rp in ([b"a"], []):
+    want_r = fr.find_rows(tape_r, str_r, rdoc[off_r:off_r + len_r], rp, rpaths, rkinds)
+    rc, N, R, index, _ = ctx.parse_find_rows(rdoc, rp, rpaths, rkinds)
+    assert rc == 0 and index.row_index.tolist() == want_r[3], (rp, index.row_index, want_r[3])
+    t_r = torch.from_numpy(tape_r.view(np.int64).copy()).cuda()
+    s_r = torch.frombuffer(bytearray(str_r), dtype=torch.uint8).cuda()
+    m_r = torch.frombuffer(bytearray(rdoc[off_r:off_r + len_r]), dtype=torch.uint8).cuda()
+    rc, N, R, index, _ = ctx.find_rows_device(t_r, s_r, m_r, rp, rpaths, rkinds)
+    assert rc == 0 and index.row_index.cpu().tolist() == want_r[3]
+nop = tape_r.copy()
+k = int(fr.find_rows(tape_r, str_r, b"", [b"a"], [], [])[3][1])  # the head of the element 3
+nop[k], nop[k + 1] = (ord("N") << 56) | 1, 0  # a nop over the number: its record is walked by one thread
+rc, N, R, index, _ = ctx.find_rows_device(torch.from_numpy(nop.view(np.int64).copy()).cuda(), s_r, m_r, [b"a"], rpaths, rkinds)
+assert rc == 0 and ctx.find_rows_serial() == 1
 # the S2 blocks of CompressFast (s2.cuh): KC1 / KC2 and KX1 / KX2 around the same calls
 from tests import s2_oracle
 ctx.set_compress_mode(1)
