@@ -310,6 +310,51 @@ __device__ __forceinline__ uint32_t fd_cvt_text(uint32_t t, uint64_t pl, uint8_t
 }
 __device__ __forceinline__ bool fd_finite(uint64_t bits) { return (bits & 0x7ff0000000000000ull) != 0x7ff0000000000000ull; }
 
+// the text of the scalar at head h, a cell of a byte column: a string's bytes are returned for the caller to copy;
+// any other scalar's StringCvt text (at most 24 bytes) is written to d, and nullptr returned
+__device__ __forceinline__ const uint8_t* fd_cell_text(const TapeView& t, uint64_t h, uint8_t* d) {
+    const uint64_t w = t.tape[h];
+    const uint32_t tag = (uint32_t)(w >> 56);
+    if (tag == '"') return tape_string_ptr(t, w);
+    fd_cvt_text<true>(tag, tape_value_tag(tag) ? t.tape[h + 1] : 0, d);
+    return nullptr;
+}
+
+// Float / Int / Uint (kind FD_FLOAT64 / FD_INT64 / FD_UINT64) of a number with tag t ('d', 'l' or 'u') and value word
+// pl: FD_OK with *v, or FD_CONVERT.  uint_max: Uint's float bound, 2^64 for Iter.Uint (parsed_json.go:679-712) but
+// float64(MaxInt64) = 2^63 for Array.AsUint64 (parsed_array.go:231-283), so there floats above 2^63 fail.
+__device__ __forceinline__ uint32_t fd_number(uint32_t t, uint64_t pl, uint32_t kind, double uint_max, uint64_t* v) {
+    const double d = __longlong_as_double((long long)pl);
+    if (kind == FD_FLOAT64) {  // Float, parsed_json.go:560-583
+        *v = t == 'd' ? pl : (uint64_t)__double_as_longlong(t == 'l' ? __ll2double_rn((long long)pl) : __ull2double_rn(pl));
+        return FD_OK;
+    }
+    if (kind == FD_INT64) {  // Int, parsed_json.go:629-661
+        if (t == 'd') {
+            // v > math.MaxInt64 compares against float64(MaxInt64) = 2^63, so exactly 2^63 passes and CVTTSD2SQ makes
+            // it math.MinInt64 (as it does NaN)
+            if (d > 9223372036854775808.0 || d < -9223372036854775808.0) return FD_CONVERT;  // "float value overflows / underflows int64"
+            *v = fd_cvttsd2sq(d);
+            return FD_OK;
+        }
+        if (t == 'u' && pl > 0x7fffffffffffffffull) return FD_CONVERT;  // "unsigned integer value overflows int64"
+        *v = pl;
+        return FD_OK;
+    }
+    // Uint
+    if (t == 'd') {
+        if (d > uint_max || d < 0) return FD_CONVERT;  // "float value overflows uint64" / "is negative"
+        // uint64(v) as Go lowers it on amd64 (cmd/compile/internal/ssagen/ssa.go, float64ToUint64):
+        //   v < 2^63 ? int64(v) : int64(v - 2^63) | 1<<63
+        // so exactly 2^64 or 2^63 (and NaN) give 1<<63, where __double2ull_rz saturates
+        *v = d < 9223372036854775808.0 ? fd_cvttsd2sq(d) : (fd_cvttsd2sq(d - 9223372036854775808.0) | 0x8000000000000000ull);
+        return FD_OK;
+    }
+    if (t == 'l' && (pl >> 63)) return FD_CONVERT;  // "int64 value is negative"
+    *v = pl;
+    return FD_OK;
+}
+
 // the accessor of `kind` on the found element e: FD_OK with *val (and the string's bytes for STRING), or its error
 __device__ uint32_t fd_convert(const FindParams& p, const FdIt& e, uint32_t kind, uint64_t* val, const uint8_t** s) {
     const uint32_t t = e.t;
@@ -342,36 +387,7 @@ __device__ uint32_t fd_convert(const FindParams& p, const FdIt& e, uint32_t kind
     }
     if (t != 'd' && t != 'l' && t != 'u') return FD_CONVERT;  // "unable to convert type %v to ..."
     if (e.off >= e.n) return FD_CORRUPT;  // "corrupt input: expected ..., but no more values on tape"
-    const uint64_t pl = p.t.tape[e.off];
-    const double d = __longlong_as_double((long long)pl);
-    if (kind == FD_FLOAT64) {  // Float, parsed_json.go:560-583
-        *val = t == 'd' ? pl : (uint64_t)__double_as_longlong(t == 'l' ? __ll2double_rn((long long)pl) : __ull2double_rn(pl));
-        return FD_OK;
-    }
-    if (kind == FD_INT64) {  // Int, parsed_json.go:629-661
-        if (t == 'd') {
-            // v > math.MaxInt64 compares against float64(MaxInt64) = 2^63, so exactly 2^63 passes and CVTTSD2SQ makes
-            // it math.MinInt64 (as it does NaN)
-            if (d > 9223372036854775808.0 || d < -9223372036854775808.0) return FD_CONVERT;
-            *val = fd_cvttsd2sq(d);
-            return FD_OK;
-        }
-        if (t == 'u' && pl > 0x7fffffffffffffffull) return FD_CONVERT;
-        *val = pl;
-        return FD_OK;
-    }
-    // Uint, parsed_json.go:679-712
-    if (t == 'd') {
-        if (d > 18446744073709551616.0 || d < 0) return FD_CONVERT;
-        // uint64(v) as Go lowers it on amd64 (cmd/compile/internal/ssagen/ssa.go, float64ToUint64):
-        //   v < 2^63 ? int64(v) : int64(v - 2^63) | 1<<63
-        // so exactly 2^64 (and NaN) give 1<<63, where __double2ull_rz saturates
-        *val = d < 9223372036854775808.0 ? fd_cvttsd2sq(d) : (fd_cvttsd2sq(d - 9223372036854775808.0) | 0x8000000000000000ull);
-        return FD_OK;
-    }
-    if (t == 'l' && (pl >> 63)) return FD_CONVERT;
-    *val = pl;
-    return FD_OK;
+    return fd_number(t, p.t.tape[e.off], kind, 18446744073709551616.0, val);
 }
 
 // KF3: one thread per cell, path-major (neighbouring threads take neighbouring rows of one path).  The block stages
@@ -525,14 +541,8 @@ __global__ void __launch_bounds__(TAPE_THREADS) fd_emit_kernel(const FindEmit p)
             col[r] = (int64_t)off;
             if (r + 1 == p.rows) col[p.rows] = (int64_t)(off + len);
             if (len && !(p.str_later >> si & 1)) {  // an OK cell: a string whose range was checked by KF3, or a scalar
-                const uint64_t h = (uint64_t)p.idx[(uint64_t)p.str_path[si] * p.rows + r];
-                const uint64_t w = p.t.tape[h];
-                if ((w >> 56) == '"') {
-                    s = tape_string_ptr(p.t, w);
-                    copy = len;
-                } else {  // STRING_CVT of a scalar: at most 24 bytes
-                    fd_cvt_text<true>((uint32_t)(w >> 56), tape_value_tag((uint32_t)(w >> 56)) ? p.t.tape[h + 1] : 0, d);
-                }
+                s = fd_cell_text(p.t, (uint64_t)p.idx[(uint64_t)p.str_path[si] * p.rows + r], d);
+                copy = s ? len : 0;
             }
         }
         fd_copy(s, d, copy);

@@ -43,6 +43,8 @@ struct FjWords {
         }
         return lo;
     }
+    // row r's first virtual word: row r's cell spans [vstart(r), vstart(r + 1))
+    __device__ __forceinline__ uint64_t vstart(uint64_t r) const { return V[cell0 + r] - v0; }
     // KM3's F over the virtual words (mj_keys_kernel)
     __device__ __forceinline__ bool f(uint64_t v, const int32_t* depth, const int32_t* par) const;
 };
@@ -56,7 +58,7 @@ struct FjWord {
 __device__ __forceinline__ FjWord fj_at(const FjWords& m, uint64_t v) {
     FjWord x;
     x.r = m.cell(v);
-    const uint64_t a = m.V[m.cell0 + x.r] - m.v0, b = m.V[m.cell0 + x.r + 1] - m.v0;
+    const uint64_t a = m.vstart(x.r), b = m.vstart(x.r + 1);
     const uint64_t lo = (uint64_t)m.head[x.r];
     x.s = MjSpan{lo, lo + (b - a), (int64_t)(lo - a)};
     x.i = v + (uint64_t)x.s.d;
@@ -128,6 +130,54 @@ __device__ __forceinline__ FjAgg fj_words_agg(const FjWords& m, uint64_t base, u
     return a;
 }
 
+// which of this thread's TAPE_ROUNDS words from `base` on are heads (bit j; a cell's first word is none), with their
+// places in x: the words of fj_words_agg, judged by KJ1's segmented head scan (tile_pre / grp_pre); numeric: every
+// other word from the one after the cell's first instead, without the scan (the heads of a numeric list's walk);
+// direct: only the heads directly inside the cell's scope (depth 1).  The whole block calls it.
+__device__ __forceinline__ uint32_t fj_heads(const FjWords& m, const FjAgg* tile_pre, const FjAgg* grp_pre, uint64_t base,
+                                             FjWord (&x)[TAPE_ROUNDS], bool numeric, bool direct) {
+    uint64_t w[TAPE_ROUNDS];
+    const FjAgg a = fj_words_agg(m, base, w, x);
+    uint32_t h = 0;
+    if (numeric) {
+#pragma unroll
+        for (int j = 0; j < TAPE_ROUNDS; j++)
+            if (base + j < m.n && !x[j].first && !((x[j].i - x[j].s.lo - 1) & 1)) h |= 1u << j;
+        return h;
+    }
+    FjAgg total;
+    FjAgg pre = agg_combine(tile_prefix(tile_pre, grp_pre, blockIdx.x), block_exclusive_scan(a, total));
+#pragma unroll
+    for (int j = 0; j < TAPE_ROUNDS; j++) {
+        if (base + j >= m.n) break;
+        if (!x[j].first && hagg_out(pre.h, 1) && (!direct || pre.h.d1 == 1)) h |= 1u << j;
+        pre = agg_combine(pre, fj_word_agg(w[j], x[j].i, x[j].first));
+    }
+    return h;
+}
+
+// a head at virtual word v that stops row r's walk lowers stop[r] to v with atomicMin (stop preset to ~0: none).  The
+// whole warp calls it for its words j: a lane's word j lies behind the lower lanes' words j, so the lowest lane of a
+// row has the warp's minimum and is the one that writes.
+__device__ __forceinline__ void fj_lower_stop(uint64_t* stop, bool stops, uint64_t r, uint64_t v) {
+    const uint32_t lane = threadIdx.x & 31;
+    const uint32_t g = __match_any_sync(FULL, stops ? r : ~0ull);
+    if (stops && !(g & ((1u << lane) - 1)) && v < *(volatile uint64_t*)&stop[r])
+        atomicMin(reinterpret_cast<unsigned long long*>(&stop[r]), (unsigned long long)v);
+}
+
+// a cell's scan in front of its first word a and behind its last word b - 1: the tile prefix (tiles of TILE words) of
+// each word's tile with the cell's in-tile prefixes c_lo / c_hi
+template <class A>
+struct FjEnds {
+    A lo, hi;
+};
+template <uint64_t TILE, class A>
+__device__ __forceinline__ FjEnds<A> fj_ends(const A* tile_pre, const A* grp_pre, const A& c_lo, const A& c_hi, uint64_t a, uint64_t b) {
+    return FjEnds<A>{agg_combine(tile_prefix(tile_pre, grp_pre, a / TILE), c_lo),
+                     agg_combine(tile_prefix(tile_pre, grp_pre, (b - 1) / TILE), c_hi)};
+}
+
 // KJ1: the segmented transfer function of each tile
 __global__ void __launch_bounds__(TAPE_THREADS) fj_heads_reduce_kernel(const FjWords m, FjAgg* tile_sum) {
     const uint64_t base = (uint64_t)blockIdx.x * TAPE_TILE + (uint64_t)threadIdx.x * TAPE_ROUNDS;
@@ -195,19 +245,18 @@ struct FjCells {
 __global__ void __launch_bounds__(256) fj_finish_kernel(const FjCells c, FindParams p) {
     const uint64_t r = (uint64_t)blockIdx.x * 256 + threadIdx.x;
     if (r >= c.m.rows) return;
-    const uint64_t a = c.m.V[c.m.cell0 + r] - c.m.v0, b = c.m.V[c.m.cell0 + r + 1] - c.m.v0;
+    const uint64_t a = c.m.vstart(r), b = c.m.vstart(r + 1);
     if (a == b) return;  // not found, or no element: KF3's status and 0 bytes stand
-    const JSum lo = agg_combine(tile_prefix(c.len_tile_pre, c.len_grp_pre, a / MJ_TILE), c.c_lo[r]);
-    const JSum hi = agg_combine(tile_prefix(c.len_tile_pre, c.len_grp_pre, (b - 1) / MJ_TILE), c.c_hi[r]);
-    uint64_t len = hi.len - lo.len;
+    const FjEnds<JSum> s = fj_ends<MJ_TILE>(c.len_tile_pre, c.len_grp_pre, c.c_lo[r], c.c_hi[r], a, b);
+    uint64_t len = s.hi.len - s.lo.len;
     const uint64_t q = (uint64_t)c.path * p.roots.n + r;
-    if (hi.bad != lo.bad || c.cbad[r]) {
+    if (s.hi.bad != s.lo.bad || c.cbad[r]) {
         p.st[q] = FD_CORRUPT;
         len = 0;
     }
     p.val[q] = len;
     p.slen[(uint64_t)c.sidx * p.roots.n + r] = len;
-    c.jbase[r] = lo.len;
+    c.jbase[r] = s.lo.len;
 }
 
 // KJ6: the words' bytes, each OK cell's at its column offset (KF5) + its place in the cell

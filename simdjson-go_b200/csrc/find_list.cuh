@@ -41,34 +41,9 @@ __device__ uint32_t fl_step(const TapeView& t, uint32_t kind, uint64_t i, uint64
         if (tag == ']') return FD_OK;
         if (tag != 'd' && tag != 'l' && tag != 'u') return FD_CONVERT;  // "unable to convert type %v to ..." (nops too)
         if (i + 1 >= hi) return FD_CORRUPT;                                // "corrupt input: ... but no more values"
-        const uint64_t pl = t.tape[i + 1];
-        const double d = __longlong_as_double((long long)pl);
-        if (kind == FD_ARRAY_FLOAT64) {
-            *v = tag == 'd' ? pl : (uint64_t)__double_as_longlong(tag == 'l' ? __ll2double_rn((long long)pl) : __ull2double_rn(pl));
-            return FL_ELEM;
-        }
-        if (kind == FD_ARRAY_INT64) {
-            if (tag == 'd') {
-                // val > math.MaxInt64 compares against float64(MaxInt64) = 2^63: exactly 2^63 (and NaN) pass and
-                // int64(val) makes them math.MinInt64 (CVTTSD2SQ)
-                if (d > 9223372036854775808.0 || d < -9223372036854775808.0) return FD_CONVERT;  // "float value overflows / underflows int64"
-                *v = fd_cvttsd2sq(d);
-                return FL_ELEM;
-            }
-            if (tag == 'u' && pl > 0x7fffffffffffffffull) return FD_CONVERT;  // "unsigned integer value overflows int64"
-            *v = pl;
-            return FL_ELEM;
-        }
-        if (tag == 'd') {
-            // unlike Iter.Uint the bound is float64(MaxInt64) = 2^63, so floats above 2^63 fail; exactly 2^63 (and NaN)
-            // pass and Go's float64ToUint64 lowering makes them 1<<63
-            if (d > 9223372036854775808.0 || d < 0) return FD_CONVERT;  // "float value overflows uint64" / "is negative"
-            *v = d < 9223372036854775808.0 ? fd_cvttsd2sq(d) : (fd_cvttsd2sq(d - 9223372036854775808.0) | 0x8000000000000000ull);
-            return FL_ELEM;
-        }
-        if (tag == 'l' && (pl >> 63)) return FD_CONVERT;  // "int64 value is negative"
-        *v = pl;
-        return FL_ELEM;
+        const uint32_t k = kind == FD_ARRAY_FLOAT64 ? FD_FLOAT64 : kind == FD_ARRAY_INT64 ? FD_INT64 : FD_UINT64;
+        // (AsUint64's float bound is float64(MaxInt64) = 2^63)
+        return fd_number(tag, t.tape[i + 1], k, 9223372036854775808.0, v) == FD_OK ? FL_ELEM : FD_CONVERT;
     }
     // AsString / AsStringCvt, parsed_array.go:287-344: AdvanceIter (parsed_json.go:291-347), then String / StringCvt
     const uint64_t cur = w & TAPE_VALUE_MASK;
@@ -119,41 +94,18 @@ struct FlCells {
 // this thread's TAPE_ROUNDS words from `base` on: their places, and which are heads the walk reads (bit j; a cell's
 // '[' is none).  The whole block calls it.
 __device__ __forceinline__ uint32_t fl_heads(const FlCells& c, uint64_t base, FjWord (&x)[TAPE_ROUNDS]) {
-    uint64_t w[TAPE_ROUNDS];
-    const FjAgg a = fj_words_agg(c.m, base, w, x);
-    uint32_t h = 0;
-    if (fl_numeric(c.kind)) {
-#pragma unroll
-        for (int j = 0; j < TAPE_ROUNDS; j++)
-            if (base + j < c.m.n && !x[j].first && !((x[j].i - x[j].s.lo - 1) & 1)) h |= 1u << j;
-        return h;
-    }
-    FjAgg total;
-    FjAgg pre = agg_combine(tile_prefix(c.h_tile_pre, c.h_grp_pre, blockIdx.x), block_exclusive_scan(a, total));
-#pragma unroll
-    for (int j = 0; j < TAPE_ROUNDS; j++) {
-        if (base + j >= c.m.n) break;
-        if (!x[j].first && hagg_out(pre.h, 1)) h |= 1u << j;
-        pre = agg_combine(pre, fj_word_agg(w[j], x[j].i, x[j].first));
-    }
-    return h;
+    return fj_heads(c.m, c.h_tile_pre, c.h_grp_pre, base, x, fl_numeric(c.kind), false);
 }
 
 // KL2: every head that stops its walk lowers the cell's stop to its word (stop preset to FL_NO_STOP)
 __global__ void __launch_bounds__(TAPE_THREADS) fl_stop_kernel(const FlCells c) {
-    const uint32_t lane = threadIdx.x & 31;
     const uint64_t base = (uint64_t)blockIdx.x * TAPE_TILE + (uint64_t)threadIdx.x * TAPE_ROUNDS;
     FjWord x[TAPE_ROUNDS];
     const uint32_t h = fl_heads(c, base, x);
 #pragma unroll
     for (int j = 0; j < TAPE_ROUNDS; j++) {
         uint64_t v;
-        const bool stops = (h >> j & 1) && fl_step(c.t, c.kind, x[j].i, x[j].s.hi, &v) != FL_ELEM;
-        const uint64_t r = stops ? x[j].r : FL_NO_STOP;
-        // a lane's word j lies behind the lower lanes' words j: the lowest lane of a cell has the warp's minimum
-        const uint32_t g = __match_any_sync(FULL, r);
-        if (stops && !(g & ((1u << lane) - 1)) && base + j < *(volatile uint64_t*)&c.stop[r])
-            atomicMin(reinterpret_cast<unsigned long long*>(&c.stop[r]), (unsigned long long)(base + j));
+        fj_lower_stop(c.stop, (h >> j & 1) && fl_step(c.t, c.kind, x[j].i, x[j].s.hi, &v) != FL_ELEM, x[j].r, base + j);
     }
 }
 
@@ -209,13 +161,9 @@ __device__ uint32_t fl_walk(const FindParams& p, uint32_t kind, uint64_t i, uint
         if (st != FL_ELEM) return st;
         if (elems) {
             elems[n->elems] = v;
-            const uint64_t w = p.t.tape[at];
-            if ((w >> 56) == '"') {
-                const uint8_t* s = tape_string_ptr(p.t, w);
+            const uint8_t* s = fd_cell_text(p.t, at, bytes + n->bytes);
+            if (s)
                 for (uint64_t b = 0; b < v; b++) bytes[n->bytes + b] = s[b];
-            } else {
-                fd_cvt_text<true>((uint32_t)(w >> 56), tape_value_tag((uint32_t)(w >> 56)) ? p.t.tape[at + 1] : 0, bytes + n->bytes);
-            }
         }
         n->elems++;
         n->bytes += v;
@@ -226,7 +174,7 @@ __device__ uint32_t fl_walk(const FindParams& p, uint32_t kind, uint64_t i, uint
 __global__ void __launch_bounds__(256) fl_finish_kernel(const FlCells c, FindParams p) {
     const uint64_t r = (uint64_t)blockIdx.x * 256 + threadIdx.x;
     if (r >= c.m.rows) return;
-    const uint64_t a = c.m.V[c.m.cell0 + r] - c.m.v0, b = c.m.V[c.m.cell0 + r + 1] - c.m.v0;
+    const uint64_t a = c.m.vstart(r), b = c.m.vstart(r + 1);
     if (a == b) return;  // no array: KF3's status, no elements and no bytes stand
     const uint64_t lo = (uint64_t)c.m.head[r], hi = lo + (b - a), s = c.stop[r];
     uint32_t st;
@@ -239,10 +187,9 @@ __global__ void __launch_bounds__(256) fl_finish_kernel(const FlCells c, FindPar
     if (fl_numeric(c.kind)) {
         if (s != FL_NO_STOP) n.elems = (s - a - 1) / 2;
     } else {
-        const LSum l = agg_combine(tile_prefix(c.l_tile_pre, c.l_grp_pre, a / TAPE_TILE), c.c_lo[r]);
-        const LSum h = agg_combine(tile_prefix(c.l_tile_pre, c.l_grp_pre, (b - 1) / TAPE_TILE), c.c_hi[r]);
-        n = LSum{h.bytes - l.bytes, h.elems - l.elems};
-        c.base[r] = l;
+        const FjEnds<LSum> e = fj_ends<TAPE_TILE>(c.l_tile_pre, c.l_grp_pre, c.c_lo[r], c.c_hi[r], a, b);
+        n = LSum{e.hi.bytes - e.lo.bytes, e.hi.elems - e.lo.elems};
+        c.base[r] = e.lo;
         c.pre[r] = n;
         if (st == FL_NOP) st = fl_walk(p, c.kind, lo + (s - a), hi, &n, nullptr, nullptr);
     }
@@ -292,13 +239,8 @@ __global__ void __launch_bounds__(TAPE_THREADS) fl_emit_kernel(const FlCells c, 
             elems[E[(uint64_t)c.lidx * rows + r] + k] = v[j];
             if (!num) {
                 d = bytes + (uint64_t)col[r] + (e.bytes - c.base[r].bytes);
-                const uint64_t w = c.t.tape[x[j].i];
-                if ((w >> 56) == '"') {
-                    s = tape_string_ptr(c.t, w);
-                    copy = v[j];
-                } else {
-                    fd_cvt_text<true>((uint32_t)(w >> 56), tape_value_tag((uint32_t)(w >> 56)) ? c.t.tape[x[j].i + 1] : 0, d);
-                }
+                s = fd_cell_text(c.t, x[j].i, d);
+                copy = s ? v[j] : 0;
             }
         }
         if (!num) {
@@ -313,7 +255,7 @@ __global__ void __launch_bounds__(256) fl_serial_emit_kernel(const FlCells c, co
                                                              const int64_t* col, uint8_t* bytes) {
     const uint64_t r = (uint64_t)blockIdx.x * 256 + threadIdx.x;
     if (r >= c.m.rows || p.st[(uint64_t)c.path * c.m.rows + r] != FD_OK) return;
-    const uint64_t a = c.m.V[c.m.cell0 + r] - c.m.v0, b = c.m.V[c.m.cell0 + r + 1] - c.m.v0, s = c.stop[r];
+    const uint64_t a = c.m.vstart(r), b = c.m.vstart(r + 1), s = c.stop[r];
     if (a == b || s == FL_NO_STOP) return;
     const uint64_t lo = (uint64_t)c.m.head[r], i = lo + (s - a);
     if ((c.t.tape[i] >> 56) != 'N') return;

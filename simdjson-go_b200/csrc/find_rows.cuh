@@ -111,37 +111,13 @@ __global__ void __launch_bounds__(256) fr_record_kernel(const FindParams p, uint
     words[r] = n;
 }
 
-// which of this thread's words are heads directly inside their array (bit j; the '[' is none), with their places
-__device__ __forceinline__ uint32_t fr_heads(const FrCells& c, uint64_t base, FjWord (&x)[TAPE_ROUNDS]) {
-    uint64_t w[TAPE_ROUNDS];
-    const FjAgg a = fj_words_agg(c.m, base, w, x);
-    FjAgg total;
-    FjAgg pre = agg_combine(tile_prefix(c.h_tile_pre, c.h_grp_pre, blockIdx.x), block_exclusive_scan(a, total));
-    uint32_t h = 0;
-#pragma unroll
-    for (int j = 0; j < TAPE_ROUNDS; j++) {
-        if (base + j >= c.m.n) break;
-        if (!x[j].first && hagg_out(pre.h, 1) && pre.h.d1 == 1) h |= 1u << j;
-        pre = agg_combine(pre, fj_word_agg(w[j], x[j].i, x[j].first));
-    }
-    return h;
-}
-
 // KR2: every head that stops its walk lowers the record's stop to its word (stop preset to FR_NO_STOP)
 __global__ void __launch_bounds__(TAPE_THREADS) fr_stop_kernel(const FrCells c) {
-    const uint32_t lane = threadIdx.x & 31;
     const uint64_t base = (uint64_t)blockIdx.x * TAPE_TILE + (uint64_t)threadIdx.x * TAPE_ROUNDS;
     FjWord x[TAPE_ROUNDS];
-    const uint32_t h = fr_heads(c, base, x);
+    const uint32_t h = fj_heads(c.m, c.h_tile_pre, c.h_grp_pre, base, x, false, true);
 #pragma unroll
-    for (int j = 0; j < TAPE_ROUNDS; j++) {
-        const bool stops = (h >> j & 1) && fr_stops(c.t, x[j].i);
-        const uint64_t r = stops ? x[j].r : FR_NO_STOP;
-        // a lane's word j lies behind the lower lanes' words j: the lowest lane of a record has the warp's minimum
-        const uint32_t g = __match_any_sync(FULL, r);
-        if (stops && !(g & ((1u << lane) - 1)) && base + j < *(volatile uint64_t*)&c.stop[r])
-            atomicMin(reinterpret_cast<unsigned long long*>(&c.stop[r]), (unsigned long long)(base + j));
-    }
+    for (int j = 0; j < TAPE_ROUNDS; j++) fj_lower_stop(c.stop, (h >> j & 1) && fr_stops(c.t, x[j].i), x[j].r, base + j);
 }
 
 // this thread's candidates (bit j: a head directly inside its array in front of the record's stop) and their RAgg
@@ -162,7 +138,7 @@ __device__ __forceinline__ uint32_t fr_cands(const FrCells& c, uint64_t base, co
 __global__ void __launch_bounds__(TAPE_THREADS) fr_count_kernel(const FrCells c, RAgg* tile) {
     const uint64_t base = (uint64_t)blockIdx.x * TAPE_TILE + (uint64_t)threadIdx.x * TAPE_ROUNDS;
     FjWord x[TAPE_ROUNDS];
-    const uint32_t h = fr_heads(c, base, x);
+    const uint32_t h = fj_heads(c.m, c.h_tile_pre, c.h_grp_pre, base, x, false, true);
     RAgg a, total;
     const uint32_t k = fr_cands(c, base, x, h, &a);
     RAgg pre = block_exclusive_scan(a, total);
@@ -180,7 +156,7 @@ __global__ void __launch_bounds__(TAPE_THREADS) fr_count_kernel(const FrCells c,
 __global__ void __launch_bounds__(TAPE_THREADS) fr_verify_kernel(const FrCells c) {
     const uint64_t base = (uint64_t)blockIdx.x * TAPE_TILE + (uint64_t)threadIdx.x * TAPE_ROUNDS;
     FjWord x[TAPE_ROUNDS];
-    const uint32_t h = fr_heads(c, base, x);
+    const uint32_t h = fj_heads(c.m, c.h_tile_pre, c.h_grp_pre, base, x, false, true);
     RAgg a;
     const uint32_t k = fr_cands(c, base, x, h, &a);
     RLast total;
@@ -217,7 +193,7 @@ __device__ uint64_t fr_walk(const TapeView& t, uint64_t lo, uint64_t hi, uint32_
 __global__ void __launch_bounds__(256) fr_finish_kernel(const FrCells c) {
     const uint64_t r = (uint64_t)blockIdx.x * 256 + threadIdx.x;
     if (r >= c.m.rows) return;
-    const uint64_t a = c.m.V[c.m.cell0 + r] - c.m.v0, b = c.m.V[c.m.cell0 + r + 1] - c.m.v0;
+    const uint64_t a = c.m.vstart(r), b = c.m.vstart(r + 1);
     c.serial[r] = 0;
     c.base[r] = 0;
     if (a == b) {  // no array: no rows
@@ -225,26 +201,25 @@ __global__ void __launch_bounds__(256) fr_finish_kernel(const FrCells c) {
         return;
     }
     const uint64_t lo = (uint64_t)c.m.head[r], hi = lo + (b - a), s = c.stop[r];
-    const RAgg l = agg_combine(tile_prefix(c.c_tile_pre, c.c_grp_pre, a / TAPE_TILE), c.c_lo[r]);
-    const RAgg e = agg_combine(tile_prefix(c.c_tile_pre, c.c_grp_pre, (b - 1) / TAPE_TILE), c.c_hi[r]);
-    uint64_t n = e.n - l.n;
+    const FjEnds<RAgg> e = fj_ends<TAPE_TILE>(c.c_tile_pre, c.c_grp_pre, c.c_lo[r], c.c_hi[r], a, b);
+    uint64_t n = e.hi.n - e.lo.n;
     bool ok = !c.bad[r];
     if (s != FR_NO_STOP) ok = ok && (c.t.tape[lo + (s - a)] >> 56) != 'N';
-    else ok = ok && (n ? fr_succ(c.t, e.last - 1 - a + lo) >= hi : lo + 1 >= hi);
+    else ok = ok && (n ? fr_succ(c.t, e.hi.last - 1 - a + lo) >= hi : lo + 1 >= hi);
     if (!ok) {
         c.serial[r] = 1;
         atomicAdd(c.n_serial, 1ull);
         n = fr_walk(c.t, lo, hi, nullptr);
     }
     c.E[r] = n;
-    c.base[r] = l.n;
+    c.base[r] = e.lo.n;
 }
 
 // KR6: each candidate of a verified record writes its row at the record's first row + its place among the candidates
 __global__ void __launch_bounds__(TAPE_THREADS) fr_emit_kernel(const FrCells c) {
     const uint64_t base = (uint64_t)blockIdx.x * TAPE_TILE + (uint64_t)threadIdx.x * TAPE_ROUNDS;
     FjWord x[TAPE_ROUNDS];
-    const uint32_t h = fr_heads(c, base, x);
+    const uint32_t h = fj_heads(c.m, c.h_tile_pre, c.h_grp_pre, base, x, false, true);
     RAgg a, total;
     const uint32_t k = fr_cands(c, base, x, h, &a);
     RAgg pre = agg_combine(tile_prefix(c.c_tile_pre, c.c_grp_pre, blockIdx.x), block_exclusive_scan(a, total));
@@ -265,7 +240,7 @@ __global__ void __launch_bounds__(TAPE_THREADS) fr_emit_kernel(const FrCells c) 
 __global__ void __launch_bounds__(256) fr_serial_emit_kernel(const FrCells c) {
     const uint64_t r = (uint64_t)blockIdx.x * 256 + threadIdx.x;
     if (r >= c.m.rows || !c.serial[r]) return;
-    const uint64_t a = c.m.V[c.m.cell0 + r] - c.m.v0, b = c.m.V[c.m.cell0 + r + 1] - c.m.v0, lo = (uint64_t)c.m.head[r];
+    const uint64_t a = c.m.vstart(r), b = c.m.vstart(r + 1), lo = (uint64_t)c.m.head[r];
     fr_walk(c.t, lo, lo + (b - a), c.erow + 2 * c.E[r]);
 }
 

@@ -140,36 +140,23 @@ class Context:
         m = _as_u8(msg)
         flags = (FLAG_NDJSON if ndjson else 0) | (FLAG_COPY_STRINGS if copy_strings else 0)
         cpaths, keep = _find_paths(paths, kinds)
-        rows, nbytes = C.c_size_t(0), C.c_size_t(0)
+        n_str, n_list = _find_counts(kinds)
+        rows, nbytes, nelems = C.c_size_t(0), C.c_size_t(0), C.c_size_t(0)
         # rows: one per record (records are separated by newlines) or the one document; strings: at most the input per
         # STRING path, guessed at its size -- else once more at the exact sizes
-        row_cap = int(np.count_nonzero(m == 10)) + 1 if ndjson else 1
-        str_cap = m.size + 64
-        n_str = sum(k in FIND_VAR_KINDS for k in kinds)
-        n_list = sum(k in FIND_LIST_KINDS for k in kinds)
-        nelems, elem_cap = C.c_size_t(0), m.size // 2 + 1
-        for _ in range(2):
-            cols = (np.empty((len(paths), row_cap), np.uint8), np.empty((len(paths), row_cap), np.uint8),
-                    np.empty((len(paths), row_cap), np.int64), np.empty((len(paths), row_cap), np.uint64),
-                    np.empty((n_str, row_cap + 1), np.int64), np.empty(max(str_cap, 1), np.uint8))
-            out = _lib.FindOut(*(_addr(a) for a in cols), row_cap, str_cap)
+        caps = (int(np.count_nonzero(m == 10)) + 1 if ndjson else 1, m.size + 64, m.size // 2 + 1 if n_list else 0)
+
+        def call(out, lout, rout):
             if n_list:
-                lcols = (np.empty((n_list, row_cap + 1), np.int64), np.empty(max(elem_cap, 1), np.uint64))
-                lout = _lib.FindListsOut(_addr(lcols[0]), _addr(lcols[1]), elem_cap)
-                rc = self.L.sj_parse_find_lists(self.h, _addr(m) if m.size else None, m.size, flags, cpaths, len(paths),
-                                                C.byref(out), C.byref(lout), C.byref(rows), C.byref(nbytes), C.byref(nelems))
-            else:
-                rc = self.L.sj_parse_find(self.h, _addr(m) if m.size else None, m.size, flags, cpaths, len(paths),
-                                          C.byref(out), C.byref(rows), C.byref(nbytes))
-            if rc != ERR_CAPACITY:
-                break
-            row_cap, str_cap, elem_cap = rows.value, nbytes.value, nelems.value
+                return self.L.sj_parse_find_lists(self.h, _addr(m) if m.size else None, m.size, flags, cpaths, len(paths), out,
+                                                  lout, C.byref(rows), C.byref(nbytes), C.byref(nelems))
+            return self.L.sj_parse_find(self.h, _addr(m) if m.size else None, m.size, flags, cpaths, len(paths), out,
+                                        C.byref(rows), C.byref(nbytes))
+        rc, cols = _find_host(call, len(paths), n_str, n_list, caps, lambda: (rows.value, nbytes.value, nelems.value))
         if rc in (ERR_STAGE1, ERR_STAGE2):
             return rc, 0, None
         if rc != OK:
             raise SjError(rc)
-        if n_list:
-            cols = cols + lcols
         return rc, rows.value, _find_columns(cols, rows.value, kinds, lambda a, dt: a.view(dt))
 
     def parse_find_rows(self, msg, row_path, paths, kinds, ndjson=True, copy_strings=True):
@@ -183,35 +170,22 @@ class Context:
         flags = (FLAG_NDJSON if ndjson else 0) | (FLAG_COPY_STRINGS if copy_strings else 0)
         cpaths, keep = _find_paths(paths, kinds)
         rpath, rkeep = _find_paths([row_path], [FIND_KIND_ELEMENT])
+        n_str, n_list = _find_counts(kinds)
         records, rows, nbytes, nelems = C.c_size_t(0), C.c_size_t(0), C.c_size_t(0), C.c_size_t(0)
-        n_str = sum(k in FIND_VAR_KINDS for k in kinds)
-        n_list = sum(k in FIND_LIST_KINDS for k in kinds)
+
+        def call(out, lout, rout):
+            return self.L.sj_parse_find_rows(self.h, _addr(m) if m.size else None, m.size, flags, rpath, cpaths, len(paths),
+                                             out, lout, rout, C.byref(records), C.byref(rows), C.byref(nbytes), C.byref(nelems))
         # the sizes first (no outputs), then the call at the exact sizes
-        rec_cap = row_cap = str_cap = elem_cap = 0
-        cols = lcols = rcols = None
-        for _ in range(2):
-            cols = (np.empty((len(paths), row_cap), np.uint8), np.empty((len(paths), row_cap), np.uint8),
-                    np.empty((len(paths), row_cap), np.int64), np.empty((len(paths), row_cap), np.uint64),
-                    np.empty((n_str, row_cap + 1), np.int64), np.empty(max(str_cap, 1), np.uint8))
-            out = _lib.FindOut(*(_addr(a) for a in cols), row_cap, str_cap)
-            lcols = (np.empty((max(n_list, 1), row_cap + 1), np.int64), np.empty(max(elem_cap, 1), np.uint64))
-            lout = _lib.FindListsOut(_addr(lcols[0]), _addr(lcols[1]), elem_cap)
-            rcols = (np.empty(max(rec_cap, 1), np.uint8), np.empty(rec_cap + 1, np.int64), np.empty(max(row_cap, 1), np.uint8),
-                     np.empty(max(row_cap, 1), np.int64))
-            rout = _lib.FindRowsOut(*(_addr(a) for a in rcols), rec_cap)
-            rc = self.L.sj_parse_find_rows(self.h, _addr(m) if m.size else None, m.size, flags, rpath, cpaths, len(paths),
-                                           C.byref(out), C.byref(lout), C.byref(rout), C.byref(records), C.byref(rows),
-                                           C.byref(nbytes), C.byref(nelems))
-            if rc != ERR_CAPACITY:
-                break
-            rec_cap, row_cap, str_cap, elem_cap = records.value, rows.value, nbytes.value, nelems.value
+        rc, cols = _find_host(call, len(paths), n_str, n_list, (0, 0, 0, 0),
+                              lambda: (rows.value, nbytes.value, nelems.value, records.value))
         if rc in (ERR_STAGE1, ERR_STAGE2):
             return rc, 0, 0, None, None
         if rc != OK:
             raise SjError(rc)
         R, n = records.value, rows.value
-        index = RowIndex(rcols[0][:R], rcols[1][:R + 1], rcols[2][:n], rcols[3][:n])
-        return rc, R, n, index, _find_columns(cols + lcols, n, kinds, lambda a, dt: a.view(dt))
+        index = RowIndex(cols[8][:R], cols[9][:R + 1], cols[10][:n], cols[11][:n])
+        return rc, R, n, index, _find_columns(cols, n, kinds, lambda a, dt: a.view(dt))
 
     def find_rows_device(self, tape, strings, message, row_path, paths, kinds, out=None):
         """Array.ForEach over every record's array at `row_path` on a tape already on this context's device (torch
@@ -219,15 +193,13 @@ class Context:
         (optional) is find_device's tuple with L list paths' two tensors always present (list_offsets [L, R + 1], elems
         [E]), then rec_status u8 [N], rec_offsets i64 [N + 1], row_tag u8 [R], row_index i64 [R]; without it the tensors
         are allocated at the exact sizes.  rc is SJ_ERR_CAPACITY when `out` is too small (the sizes are still exact)."""
-        import torch
         cpaths, keep = _find_paths(paths, kinds)
         rpath, rkeep = _find_paths([row_path], [FIND_KIND_ELEMENT])
+        n_str, n_list = _find_counts(kinds)
         sp, sl = _ptr_len(strings)
         mp, ml = _ptr_len(message)
         tp, tl = _ptr_len(tape)
         records, rows, nbytes, nelems = C.c_size_t(0), C.c_size_t(0), C.c_size_t(0), C.c_size_t(0)
-        n_str = sum(k in FIND_VAR_KINDS for k in kinds)
-        n_list = sum(k in FIND_LIST_KINDS for k in kinds)
 
         def call(o, lo, ro):
             return self.L.sj_find_rows_device(self.h, mp, ml, tp, tl, sp, sl, rpath, cpaths, len(paths), o, lo, ro,
@@ -236,14 +208,8 @@ class Context:
             rc = call(None, None, None)
             if rc not in (OK, ERR_CAPACITY):
                 return rc, records.value, rows.value, None, None
-            dev, N, R = tape.device, records.value, rows.value
-            u8, i64 = torch.uint8, torch.int64
-            out = (torch.empty((len(paths), R), dtype=u8, device=dev), torch.empty((len(paths), R), dtype=u8, device=dev),
-                   torch.empty((len(paths), R), dtype=i64, device=dev), torch.empty((len(paths), R), dtype=i64, device=dev),
-                   torch.empty((n_str, R + 1), dtype=i64, device=dev), torch.empty(max(nbytes.value, 1), dtype=u8, device=dev),
-                   torch.empty((n_list, R + 1), dtype=i64, device=dev), torch.empty(max(nelems.value, 1), dtype=i64, device=dev),
-                   torch.empty(max(N, 1), dtype=u8, device=dev), torch.empty(N + 1, dtype=i64, device=dev),
-                   torch.empty(max(R, 1), dtype=u8, device=dev), torch.empty(max(R, 1), dtype=i64, device=dev))
+            out = _find_cols(_torch_empty(tape.device), len(paths), n_str, n_list, rows.value, nbytes.value, nelems.value,
+                             records.value)
         if len(out) != 12:
             raise ValueError("find_rows_device: out needs 12 tensors")
         row_cap = out[0].shape[1]
@@ -254,9 +220,7 @@ class Context:
         rec_cap = out[9].numel() - 1
         if out[8].numel() < rec_cap or out[10].numel() < row_cap or out[11].numel() < row_cap:
             raise ValueError("find_rows_device: record and row columns smaller than their caps")
-        o = _lib.FindOut(*(t.data_ptr() for t in out[:6]), row_cap, out[5].numel())
-        lo = _lib.FindListsOut(out[6].data_ptr(), out[7].data_ptr(), out[7].numel())
-        ro = _lib.FindRowsOut(*(t.data_ptr() for t in out[8:12]), rec_cap)
+        o, lo, ro = _find_outs(out, _data_ptr, row_cap, out[5].numel(), out[7].numel(), rec_cap)
         rc = call(C.byref(o), C.byref(lo), C.byref(ro))
         N, R = records.value, rows.value
         if rc != OK:
@@ -281,15 +245,12 @@ class Context:
         FLOAT64 and uint64 for UINT64, elems as float64 / int64 / uint64 by list kind), or None unless rc is OK.  rc is
         SJ_ERR_CAPACITY when `out` is too small (rows and the byte total are still exact, in `rows` and nothing written).
         Without list kinds the call is sj_find_device."""
-        import torch
         cpaths, keep = _find_paths(paths, kinds)
+        n_str, n_list = _find_counts(kinds)
         sp, sl = _ptr_len(strings)
         mp, ml = _ptr_len(message)
         tp, tl = _ptr_len(tape)
-        rows, nbytes = C.c_size_t(0), C.c_size_t(0)
-        n_str = sum(k in FIND_VAR_KINDS for k in kinds)
-        n_list = sum(k in FIND_LIST_KINDS for k in kinds)
-        nelems = C.c_size_t(0)
+        rows, nbytes, nelems = C.c_size_t(0), C.c_size_t(0), C.c_size_t(0)
 
         def call(o, lo):
             if n_list:
@@ -300,13 +261,8 @@ class Context:
             rc = call(None, None)
             if rc not in (OK, ERR_CAPACITY):
                 return rc, rows.value, None
-            dev, R = tape.device, rows.value
-            out = (torch.empty((len(paths), R), dtype=torch.uint8, device=dev), torch.empty((len(paths), R), dtype=torch.uint8, device=dev),
-                   torch.empty((len(paths), R), dtype=torch.int64, device=dev), torch.empty((len(paths), R), dtype=torch.int64, device=dev),
-                   torch.empty((n_str, R + 1), dtype=torch.int64, device=dev), torch.empty(max(nbytes.value, 1), dtype=torch.uint8, device=dev))
-            if n_list:
-                out += (torch.empty((n_list, R + 1), dtype=torch.int64, device=dev),
-                        torch.empty(max(nelems.value, 1), dtype=torch.int64, device=dev))
+            out = _find_cols(_torch_empty(tape.device), len(paths), n_str, n_list, rows.value, nbytes.value,
+                             nelems.value)[:8 if n_list else 6]
         row_cap = out[0].shape[1]
         shapes = [(len(paths), row_cap)] * 4 + [(n_str, row_cap + 1)] + ([(n_list, row_cap + 1)] if n_list else [])
         for t, shape in zip(out[:5] + out[6:7], shapes):
@@ -314,8 +270,7 @@ class Context:
                 raise ValueError("find_device: out tensors must be contiguous with shapes %s" % shape)
         if len(out) != (8 if n_list else 6):
             raise ValueError("find_device: out needs %d tensors" % (8 if n_list else 6))
-        o = _lib.FindOut(*(t.data_ptr() for t in out[:6]), row_cap, out[5].numel())
-        lo = _lib.FindListsOut(out[6].data_ptr(), out[7].data_ptr(), out[7].numel()) if n_list else None
+        o, lo, _ = _find_outs(out, _data_ptr, row_cap, out[5].numel(), out[7].numel() if n_list else 0)
         rc = call(C.byref(o), C.byref(lo) if n_list else None)
         if rc != OK:
             return rc, rows.value, None
@@ -643,6 +598,58 @@ def _find_paths(paths, kinds):
         keep += [blob, lens]
         arr[i] = _lib.FindPath(C.cast(blob, C.c_void_p), lens, len(segs), int(kind))
     return arr, keep
+
+
+def _find_counts(kinds):
+    """the paths with a byte column and the list paths"""
+    return sum(k in FIND_VAR_KINDS for k in kinds), sum(k in FIND_LIST_KINDS for k in kinds)
+
+
+def _find_cols(empty, n_paths, n_str, n_list, row_cap, str_cap, elem_cap, rec_cap=None):
+    """a find's columns at the given capacities, each empty(shape, numpy dtype): status, tag, index, value [paths, row_cap],
+    str_offsets [n_str, row_cap + 1], str_bytes [str_cap], list_offsets [n_list, row_cap + 1], elems [elem_cap]; with
+    rec_cap the array rows' rec_status [rec_cap], rec_offsets [rec_cap + 1], row_tag and row_index [row_cap] behind them"""
+    P = n_paths
+    cols = (empty((P, row_cap), np.uint8), empty((P, row_cap), np.uint8), empty((P, row_cap), np.int64),
+            empty((P, row_cap), np.uint64), empty((n_str, row_cap + 1), np.int64), empty(max(str_cap, 1), np.uint8),
+            empty((n_list, row_cap + 1), np.int64), empty(max(elem_cap, 1), np.uint64))
+    if rec_cap is not None:
+        cols += (empty(max(rec_cap, 1), np.uint8), empty(rec_cap + 1, np.int64), empty(max(row_cap, 1), np.uint8),
+                 empty(max(row_cap, 1), np.int64))
+    return cols
+
+
+def _find_outs(cols, ptr, row_cap, str_cap, elem_cap, rec_cap=None):
+    """the sj_find_out, sj_find_lists_out (None for 6 columns) and sj_find_rows_out (None without rec_cap) over
+    _find_cols' columns, ptr(column) their addresses"""
+    out = _lib.FindOut(*(ptr(a) for a in cols[:6]), row_cap, str_cap)
+    lout = _lib.FindListsOut(ptr(cols[6]), ptr(cols[7]), elem_cap) if len(cols) > 6 else None
+    rout = _lib.FindRowsOut(*(ptr(a) for a in cols[8:12]), rec_cap) if rec_cap is not None else None
+    return out, lout, rout
+
+
+def _find_host(call, n_paths, n_str, n_list, caps, sizes):
+    """call(out, lists, rows_out) into numpy columns at caps = (row_cap, str_cap, elem_cap[, rec_cap]), and once more at
+    the exact sizes() when that returns ERR_CAPACITY: (rc, columns)"""
+    for _ in range(2):
+        cols = _find_cols(np.empty, n_paths, n_str, n_list, *caps)
+        outs = _find_outs(cols, _addr, *caps)
+        rc = call(*(C.byref(o) if o is not None else None for o in outs))
+        if rc != ERR_CAPACITY:
+            break
+        caps = sizes()
+    return rc, cols
+
+
+def _data_ptr(t):
+    return t.data_ptr()
+
+
+def _torch_empty(dev):
+    """empty(shape, numpy dtype) for _find_cols: torch tensors on dev (int64 for the uint64 columns)"""
+    import torch
+    dt = {np.uint8: torch.uint8, np.int64: torch.int64, np.uint64: torch.int64}
+    return lambda shape, d: torch.empty(shape, dtype=dt[d], device=dev)
 
 
 def _torch_view(a, dt):
