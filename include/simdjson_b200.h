@@ -355,9 +355,53 @@ int sj_find_rows_device(sj_ctx* ctx, const uint8_t* d_msg, size_t msg_len, const
 int sj_parse_find_rows(sj_ctx* ctx, const uint8_t* msg, size_t len, uint32_t flags, const sj_find_path* row_path,
                        const sj_find_path* paths, size_t n_paths, const sj_find_out* out, const sj_find_lists_out* lists,
                        const sj_find_rows_out* rows_out, size_t* records, size_t* rows, size_t* str_bytes, size_t* elems);
-/* test hook: how many records of this context's last array-rows call failed the propose / verify checks and were
- * walked by one thread (0 on every tape the parser writes) */
+/* test hook: how many records of this context's last array-rows or member-rows call failed the propose / verify checks
+ * and were walked by one thread (0 on every tape the parser writes) */
 int sj_test_find_rows_serial(sj_ctx* ctx, uint64_t* records);
+
+/*
+ * Member rows of the find: Object.ForEach over every record's object at a row path, each member one row of the find's
+ * columns, with its key in a column of its own.  Records as for the array rows, with Element.Iter.Object
+ * (parsed_json.go:998-1018) in place of Iter.Array: SJ_FIND_CONVERT "next item is not object" or a fresh Element;
+ * SJ_FIND_CORRUPT "object ends at index before start" or "object extended beyond tape".  A row path of 0 segments takes
+ * elem.Object directly (root objects, NDJSON records: every key of every record).
+ * Rows: the members for which Object.ForEach(fn, onlyKeys) (parsed_object.go:142-186) calls fn, in order, over the
+ * object's tape Tape[:end] with Advance: a key position or a value of TypeNone ('}', ']', an unknown tag, a scope whose
+ * link lies behind it, the end of the tape) ends the walk silently, a nop is skipped as Advance skips it, a key that is
+ * not a string or has no two words behind it inside the tape ("unexpected name tag") or whose bytes lie outside their
+ * buffer ("getting object name") makes the record SJ_FIND_CORRUPT.  The rows fn received in front of that error stay:
+ * this is the one case where a record that is not OK has rows.  only_keys (kind SJ_FIND_KIND_ELEMENT, a path's limits:
+ * at most 32 keys, 16 KiB; NULL or 0 segments: every key) is onlyKeys: a member whose key is not among its segments is
+ * skipped, and the walk ends at the match whose count equals the number of distinct segments (matches are counted, so a
+ * key that occurs twice is two rows).
+ * Cells: a path of >= 1 segment is the array rows' cell from the Iter fn receives; a path of 0 segments is the member's
+ * value itself, the element Object.FindPath returns when it stops at this member (AdvanceIter from the key,
+ * parsed_object.go:298-303), with every kind applied to it.  rows_out is the array rows' layout with row_tag / row_index
+ * of each member's value head.
+ * Keys (sj_find_keys_out): row r's key is key_bytes[key_offsets[r], key_offsets[r + 1]), unescaped as stringByteAt
+ * returns it (from Strings.B, or from the message for no-copy strings); key_offsets has row_cap + 1 entries (key_offsets[0]
+ * = 0, also with no rows).  *records, *rows, *str_bytes, *elems and *key_bytes are exact even on SJ_ERR_CAPACITY (also
+ * key_bytes > key_cap), when nothing is written; every output may be NULL to ask for the sizes.  The object words of all
+ * records above SJ_MAX_MARSHAL_TAPE return SJ_ERR_TOO_LARGE.
+ * The enumeration is the array rows' over the object words; each candidate's rank in its record tells key from value,
+ * and the selected keys are counted by a scan of their own.  Launches: the array rows' with 3 more over the object words
+ * (KO1 and its scan), KO2 in place of KR6, and for rows > 0 4 for the key lengths' scan with a read-back and KO3.
+ * sj_find_members_device: as sj_find_rows_device (device memory).  sj_parse_find_members: as sj_parse_find_rows.
+ */
+typedef struct {
+    int64_t* key_offsets;  /* [row_cap + 1]: row r's key is key_bytes[key_offsets[r] .. key_offsets[r + 1]) */
+    uint8_t* key_bytes;    /* key_cap bytes */
+    size_t key_cap;
+} sj_find_keys_out;
+int sj_find_members_device(sj_ctx* ctx, const uint8_t* d_msg, size_t msg_len, const uint64_t* d_tape, size_t tape_len,
+                           const uint8_t* d_strings, size_t strings_len, const sj_find_path* row_path,
+                           const sj_find_path* only_keys, const sj_find_path* paths, size_t n_paths, const sj_find_out* out,
+                           const sj_find_lists_out* lists, const sj_find_rows_out* rows_out, const sj_find_keys_out* keys_out,
+                           size_t* records, size_t* rows, size_t* str_bytes, size_t* elems, size_t* key_bytes);
+int sj_parse_find_members(sj_ctx* ctx, const uint8_t* msg, size_t len, uint32_t flags, const sj_find_path* row_path,
+                          const sj_find_path* only_keys, const sj_find_path* paths, size_t n_paths, const sj_find_out* out,
+                          const sj_find_lists_out* lists, const sj_find_rows_out* rows_out, const sj_find_keys_out* keys_out,
+                          size_t* records, size_t* rows, size_t* str_bytes, size_t* elems, size_t* key_bytes);
 
 /*
  * MarshalJSON on the device: Iter.MarshalJSON of a fresh pj.Iter() (parsed_json.go:394-556), byte for byte.  Every

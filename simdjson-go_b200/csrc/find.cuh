@@ -60,7 +60,7 @@ struct FdSeg {
 struct FindParams {
     TapeView t;
     TapeRows roots;          // one row per root; with element rows (find_rows.cuh) roots.n is their count
-    const uint32_t* erow;    // element rows: (head, array end) of row r at 2r, 2r + 1
+    const uint32_t* erow;    // element or member rows: (head, container end) of row r at 2r, 2r + 1
     uint32_t n_paths;
     const FdPath* paths;
     const FdSeg* segs;
@@ -73,6 +73,7 @@ struct FindParams {
     uint64_t* slen;          // variable-length cells: bytes of the string or text (0 unless OK), at sidx * rows + r
     uint64_t* jlen;          // JSON and list cells: tape words of the found element (0 unless found), at jidx * rows + r
     uint64_t* ecnt;          // list cells: elements (0 unless OK), at lidx * rows + r
+    const uint32_t* krow;    // member rows (an object's members, find_rows.cuh): the key head of row r; else nullptr
 };
 
 // the Iter fields the walk uses (parsed_json.go:180-195); n = length of its restricted tape
@@ -392,7 +393,8 @@ __device__ uint32_t fd_convert(const FindParams& p, const FdIt& e, uint32_t kind
 
 // KF3: one thread per cell, path-major (neighbouring threads take neighbouring rows of one path).  The block stages
 // the segments of the paths its cells belong to: their descriptors, then their bytes.  ELEMS: the rows are array
-// elements (find_rows.cuh), each an Iter that Array.ForEach's Advance left on the element's head, over the array's tape.
+// elements or an object's members (find_rows.cuh), each an Iter that ForEach's Advance left on the element's (the
+// member value's) head, over the container's tape.
 template <bool ELEMS>
 __global__ void __launch_bounds__(FD_THREADS) fd_walk_kernel(const FindParams p) {
     extern __shared__ uint8_t fd_smem[];
@@ -422,7 +424,16 @@ __global__ void __launch_bounds__(FD_THREADS) fd_walk_kernel(const FindParams p)
         const uint64_t h = p.erow[2 * r], w = p.t.tape[h];
         FdIt cp{p.erow[2 * r + 1], h + 1, 0, w & TAPE_VALUE_MASK, (uint32_t)(w >> 56)};
         fd_calc_next(cp, false);
-        st = fd_find_element(p, cp, sseg + (path.seg0 - s_lo), sbytes, path.nseg, e, &fresh);
+        if (path.nseg == 0 && p.krow) {  // a member's value: the element Object.FindPath returns when it stops at the
+                                         // member's key (AdvanceIter from the key, parsed_object.go:298-303)
+            FdIt k{cp.n, (uint64_t)p.krow[r] + 1, 1, 0, '"'};
+            uint32_t t;
+            st = fd_advance_iter(p, k, e, &t);
+            fresh = st == FD_NOT_FOUND;
+            if (fresh) st = FD_OK;
+        } else {
+            st = fd_find_element(p, cp, sseg + (path.seg0 - s_lo), sbytes, path.nseg, e, &fresh);
+        }
     } else {
         st = fd_find(p, tape_root(p.roots, r), sseg + (path.seg0 - s_lo), sbytes, path.nseg, e, &fresh);
     }

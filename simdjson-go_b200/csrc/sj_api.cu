@@ -11,6 +11,8 @@
 #include <cstdlib>
 #include <cstring>
 #include <new>
+#include <set>
+#include <string>
 #include <vector>
 
 #include <sched.h>

@@ -228,8 +228,83 @@ class Context:
         index = RowIndex(out[8][:N], out[9][:N + 1], out[10][:R], out[11][:R])
         return rc, N, R, index, _find_columns(out, R, kinds, _torch_view)
 
+    def parse_find_members(self, msg, row_path, paths, kinds, only_keys=None, ndjson=True, copy_strings=True):
+        """parseMessage, then Object.ForEach(fn, onlyKeys) over every record's object at `row_path` (a key path; [] takes
+        the record itself, so every key of every NDJSON record), each member fn receives one row of parse_find's
+        columns: (rc, records, rows, MemberIndex, columns).  A path of >= 1 segment is FindElement(path...) from the
+        member's Iter; a path of 0 segments is the member's value itself.  `only_keys` (a list of byte strings, None or
+        [] for every key) is onlyKeys.  MemberIndex is RowIndex (row_tag / row_index of each member's value head) with
+        each row's key: key(r), or key_data[key_offsets[r]:key_offsets[r + 1]].  A record whose ForEach returned an
+        error is SJ_FIND_CORRUPT and keeps the rows in front of the error.  On a parse error records and rows are 0
+        and MemberIndex and columns are None."""
+        m = _as_u8(msg)
+        flags = (FLAG_NDJSON if ndjson else 0) | (FLAG_COPY_STRINGS if copy_strings else 0)
+        cpaths, keep = _find_paths(paths, kinds)
+        rpath, rkeep = _find_paths([row_path, only_keys or []], [FIND_KIND_ELEMENT] * 2)
+        n_str, n_list = _find_counts(kinds)
+        records, rows, nbytes, nelems, nkeys = (C.c_size_t(0) for _ in range(5))
+
+        def call(out, lout, rout, kout):
+            return self.L.sj_parse_find_members(self.h, _addr(m) if m.size else None, m.size, flags, rpath,
+                                                C.pointer(rpath[1]), cpaths, len(paths), out, lout,
+                                                rout, kout, C.byref(records), C.byref(rows), C.byref(nbytes),
+                                                C.byref(nelems), C.byref(nkeys))
+        # the sizes first (no outputs), then the call at the exact sizes
+        rc, cols = _find_host(call, len(paths), n_str, n_list, (0, 0, 0, 0, 0),
+                              lambda: (rows.value, nbytes.value, nelems.value, records.value, nkeys.value))
+        if rc in (ERR_STAGE1, ERR_STAGE2):
+            return rc, 0, 0, None, None
+        if rc != OK:
+            raise SjError(rc)
+        R, n = records.value, rows.value
+        index = MemberIndex(cols[8][:R], cols[9][:R + 1], cols[10][:n], cols[11][:n], cols[12][:n + 1], cols[13][:nkeys.value])
+        return rc, R, n, index, _find_columns(cols, n, kinds, lambda a, dt: a.view(dt))
+
+    def find_members_device(self, tape, strings, message, row_path, paths, kinds, only_keys=None, out=None):
+        """Object.ForEach over every record's object at `row_path` on a tape already on this context's device (torch
+        tensors as for find_device): (rc, records, rows, MemberIndex, columns) as parse_find_members, of tensor views.
+        `out` (optional) is find_rows_device's 12 tensors, then key_offsets i64 [R + 1] and key_bytes u8 [K]; without
+        it the tensors are allocated at the exact sizes.  rc is SJ_ERR_CAPACITY when `out` is too small (the sizes are
+        still exact)."""
+        cpaths, keep = _find_paths(paths, kinds)
+        rpath, rkeep = _find_paths([row_path, only_keys or []], [FIND_KIND_ELEMENT] * 2)
+        n_str, n_list = _find_counts(kinds)
+        sp, sl = _ptr_len(strings)
+        mp, ml = _ptr_len(message)
+        tp, tl = _ptr_len(tape)
+        records, rows, nbytes, nelems, nkeys = (C.c_size_t(0) for _ in range(5))
+
+        def call(o, lo, ro, ko):
+            return self.L.sj_find_members_device(self.h, mp, ml, tp, tl, sp, sl, rpath, C.pointer(rpath[1]),
+                                                 cpaths, len(paths), o, lo, ro, ko, C.byref(records), C.byref(rows),
+                                                 C.byref(nbytes), C.byref(nelems), C.byref(nkeys))
+        if out is None:
+            rc = call(None, None, None, None)
+            if rc not in (OK, ERR_CAPACITY):
+                return rc, records.value, rows.value, None, None
+            out = _find_cols(_torch_empty(tape.device), len(paths), n_str, n_list, rows.value, nbytes.value, nelems.value,
+                             records.value, nkeys.value)
+        if len(out) != 14:
+            raise ValueError("find_members_device: out needs 14 tensors")
+        row_cap = out[0].shape[1]
+        shapes = [(len(paths), row_cap)] * 4 + [(n_str, row_cap + 1), None, (n_list, row_cap + 1)]
+        for t, shape in zip(out, shapes):
+            if (shape is not None and tuple(t.shape) != shape) or not t.is_contiguous():
+                raise ValueError("find_members_device: out tensors must be contiguous with shapes %s" % shape)
+        rec_cap = out[9].numel() - 1
+        if out[8].numel() < rec_cap or out[10].numel() < row_cap or out[11].numel() < row_cap or out[12].numel() != row_cap + 1:
+            raise ValueError("find_members_device: record, row and key columns do not match their caps")
+        o, lo, ro, ko = _find_outs(out, _data_ptr, row_cap, out[5].numel(), out[7].numel(), rec_cap, out[13].numel())
+        rc = call(C.byref(o), C.byref(lo), C.byref(ro), C.byref(ko))
+        N, R = records.value, rows.value
+        if rc != OK:
+            return rc, N, R, None, None
+        index = MemberIndex(out[8][:N], out[9][:N + 1], out[10][:R], out[11][:R], out[12][:R + 1], out[13][:nkeys.value])
+        return rc, N, R, index, _find_columns(out, R, kinds, _torch_view)
+
     def find_rows_serial(self):
-        """test hook: the records of the last array-rows call whose rows one thread walked (sj_test_find_rows_serial)"""
+        """test hook: the records of the last array-rows or member-rows call whose rows one thread walked
+        (sj_test_find_rows_serial)"""
         n = C.c_uint64(0)
         if self.L.sj_test_find_rows_serial(self.h, C.byref(n)) != OK:
             raise SjError(ERR_ARGUMENT)
@@ -585,6 +660,22 @@ class RowIndex(tuple):
     row_index = property(lambda s: s[3])
 
 
+class MemberIndex(RowIndex):
+    """the records and rows of a find over member rows: RowIndex's fields (row_tag and row_index of each member's value
+    head), then key_offsets and key_data: row r's key is key_data[key_offsets[r]:key_offsets[r + 1]]"""
+    __slots__ = ()
+    _fields = RowIndex._fields + ("key_offsets", "key_data")
+
+    key_offsets = property(lambda s: s[4])
+    key_data = property(lambda s: s[5])
+
+    def key(self, r):
+        """row r's key as bytes"""
+        a, b = int(self.key_offsets[r]), int(self.key_offsets[r + 1])
+        d = self.key_data[a:b]
+        return bytes(d.cpu().numpy() if hasattr(d, "cpu") else d)
+
+
 def _find_paths(paths, kinds):
     """the sj_find_path array (and the buffers it points into)"""
     if len(paths) != len(kinds):
@@ -605,10 +696,11 @@ def _find_counts(kinds):
     return sum(k in FIND_VAR_KINDS for k in kinds), sum(k in FIND_LIST_KINDS for k in kinds)
 
 
-def _find_cols(empty, n_paths, n_str, n_list, row_cap, str_cap, elem_cap, rec_cap=None):
+def _find_cols(empty, n_paths, n_str, n_list, row_cap, str_cap, elem_cap, rec_cap=None, key_cap=None):
     """a find's columns at the given capacities, each empty(shape, numpy dtype): status, tag, index, value [paths, row_cap],
     str_offsets [n_str, row_cap + 1], str_bytes [str_cap], list_offsets [n_list, row_cap + 1], elems [elem_cap]; with
-    rec_cap the array rows' rec_status [rec_cap], rec_offsets [rec_cap + 1], row_tag and row_index [row_cap] behind them"""
+    rec_cap the array rows' rec_status [rec_cap], rec_offsets [rec_cap + 1], row_tag and row_index [row_cap] behind them,
+    and with key_cap the member rows' key_offsets [row_cap + 1] and key_bytes [key_cap] behind those"""
     P = n_paths
     cols = (empty((P, row_cap), np.uint8), empty((P, row_cap), np.uint8), empty((P, row_cap), np.int64),
             empty((P, row_cap), np.uint64), empty((n_str, row_cap + 1), np.int64), empty(max(str_cap, 1), np.uint8),
@@ -616,21 +708,25 @@ def _find_cols(empty, n_paths, n_str, n_list, row_cap, str_cap, elem_cap, rec_ca
     if rec_cap is not None:
         cols += (empty(max(rec_cap, 1), np.uint8), empty(rec_cap + 1, np.int64), empty(max(row_cap, 1), np.uint8),
                  empty(max(row_cap, 1), np.int64))
+    if key_cap is not None:
+        cols += (empty(row_cap + 1, np.int64), empty(max(key_cap, 1), np.uint8))
     return cols
 
 
-def _find_outs(cols, ptr, row_cap, str_cap, elem_cap, rec_cap=None):
+def _find_outs(cols, ptr, row_cap, str_cap, elem_cap, rec_cap=None, key_cap=None):
     """the sj_find_out, sj_find_lists_out (None for 6 columns) and sj_find_rows_out (None without rec_cap) over
-    _find_cols' columns, ptr(column) their addresses"""
+    _find_cols' columns, ptr(column) their addresses; with key_cap the sj_find_keys_out behind them"""
     out = _lib.FindOut(*(ptr(a) for a in cols[:6]), row_cap, str_cap)
     lout = _lib.FindListsOut(ptr(cols[6]), ptr(cols[7]), elem_cap) if len(cols) > 6 else None
     rout = _lib.FindRowsOut(*(ptr(a) for a in cols[8:12]), rec_cap) if rec_cap is not None else None
-    return out, lout, rout
+    if key_cap is None:
+        return out, lout, rout
+    return out, lout, rout, _lib.FindKeysOut(ptr(cols[12]), ptr(cols[13]), key_cap)
 
 
 def _find_host(call, n_paths, n_str, n_list, caps, sizes):
-    """call(out, lists, rows_out) into numpy columns at caps = (row_cap, str_cap, elem_cap[, rec_cap]), and once more at
-    the exact sizes() when that returns ERR_CAPACITY: (rc, columns)"""
+    """call(out, lists, rows_out[, keys_out]) into numpy columns at caps = (row_cap, str_cap, elem_cap[, rec_cap[,
+    key_cap]]), and once more at the exact sizes() when that returns ERR_CAPACITY: (rc, columns)"""
     for _ in range(2):
         cols = _find_cols(np.empty, n_paths, n_str, n_list, *caps)
         outs = _find_outs(cols, _addr, *caps)

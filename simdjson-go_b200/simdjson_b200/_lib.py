@@ -21,7 +21,7 @@ EXPORTS = [
     "sj_host_free", "sj_trim_space", "sj_bounds", "sj_parse", "sj_parse_device", "sj_gen_ndjson_device", "sj_parse_nd_sharded_count", "sj_parse_nd_sharded_emit", "sj_exchange_create", "sj_exchange_set_gap", "sj_exchange_set_timeout_ms", "sj_exchange_connect", "sj_exchange_connect_ptrs", "sj_exchange_local", "sj_exchange_bases", "sj_exchange_result", "sj_find_structural_indices", "sj_stage1_device",
     "sj_stage1_launch", "sj_ctx_sync", "sj_event_record", "sj_event_elapsed_ms", "sj_kernel_launches",
     "sj_test_block_masks", "sj_test_geometry", "sj_test_finalize", "sj_test_flatten_bits", "sj_test_parse_strings",
-    "sj_test_parse_numbers", "sj_count_where_device", "sj_parse_count_where", "sj_find_device", "sj_parse_find", "sj_find_lists_device", "sj_parse_find_lists", "sj_find_rows_device", "sj_parse_find_rows", "sj_test_find_rows_serial", "sj_marshal_device", "sj_parse_marshal", "sj_serialize_device", "sj_parse_serialize",
+    "sj_test_parse_numbers", "sj_count_where_device", "sj_parse_count_where", "sj_find_device", "sj_parse_find", "sj_find_lists_device", "sj_parse_find_lists", "sj_find_rows_device", "sj_parse_find_rows", "sj_find_members_device", "sj_parse_find_members", "sj_test_find_rows_serial", "sj_marshal_device", "sj_parse_marshal", "sj_serialize_device", "sj_parse_serialize",
     "sj_deserialize_device", "sj_test_set_string_hash_bits", "sj_ctx_set_compress_mode", "sj_test_s2_encode", "sj_test_s2_decode", "sj_test_zstd_encode", "sj_test_zstd_decode", "sj_test_stage2_internal", "sj_test_stage1_ctas", "sj_stream_create", "sj_stream_destroy",
     "sj_stream_write", "sj_stream_close_input", "sj_stream_next", "sj_stream_release",
 ]
@@ -67,6 +67,10 @@ class FindListsOut(C.Structure):
 class FindRowsOut(C.Structure):
     _fields_ = [("rec_status", C.c_void_p), ("rec_offsets", C.c_void_p), ("row_tag", C.c_void_p), ("row_index", C.c_void_p),
                 ("record_cap", C.c_size_t)]
+
+
+class FindKeysOut(C.Structure):
+    _fields_ = [("key_offsets", C.c_void_p), ("key_bytes", C.c_void_p), ("key_cap", C.c_size_t)]
 
 
 class Stage1Info(C.Structure):
@@ -181,6 +185,14 @@ def load():
     L.sj_parse_find_rows.restype = i32
     L.sj_parse_find_rows.argtypes = [vp, vp, sz, u32, C.POINTER(FindPath), C.POINTER(FindPath), sz, C.POINTER(FindOut),
                                      C.POINTER(FindListsOut), C.POINTER(FindRowsOut), szp, szp, szp, szp]
+    L.sj_find_members_device.restype = i32
+    L.sj_find_members_device.argtypes = [vp, vp, sz, vp, sz, vp, sz, C.POINTER(FindPath), C.POINTER(FindPath), C.POINTER(FindPath), sz,
+                                         C.POINTER(FindOut), C.POINTER(FindListsOut), C.POINTER(FindRowsOut), C.POINTER(FindKeysOut),
+                                         szp, szp, szp, szp, szp]
+    L.sj_parse_find_members.restype = i32
+    L.sj_parse_find_members.argtypes = [vp, vp, sz, u32, C.POINTER(FindPath), C.POINTER(FindPath), C.POINTER(FindPath), sz,
+                                        C.POINTER(FindOut), C.POINTER(FindListsOut), C.POINTER(FindRowsOut), C.POINTER(FindKeysOut),
+                                        szp, szp, szp, szp, szp]
     L.sj_test_find_rows_serial.restype = i32
     L.sj_test_find_rows_serial.argtypes = [vp, C.POINTER(u64)]
     L.sj_marshal_device.restype = i32

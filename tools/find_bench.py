@@ -31,8 +31,18 @@ element):
   rows_ms, launches per call, records, rows, bytes and elements out, records walked by one thread, and min_bytes
   (the array words read once, the record and row columns, the cells, bytes and elements written) over rows_ms as a
   fraction of 3.35 TB/s
+Then one JSON line per member-rows workload (sj_find_members_device: every record's object at a row path, one row per
+member, with its key):
+  plugins           {"plugins": {...}}: update-center's plugins with their keys made unique, repeated to --mib, row path
+                    ["plugins"]: ["version"] STRING, ["url"] STRING, [] JSON (the member's value), each alone and all
+  events            citm_catalog's events, the same way: ["name"] STRING, [] JSON, each alone and both
+  K0 explode        the K0 batch at --mib, row path [] (every key of every record): [] STRING_CVT with every key, and
+                    with two only_keys
+  members_ms, launches per call, records, rows, key bytes, bytes out, records walked by one thread, the object words,
+  and min_bytes (the object words read once, the record, row and key columns, the cells and bytes written) over
+  members_ms as a fraction of 3.35 TB/s, beside sj_marshal_device of the same tape
 The card's name and power limit are read in the same run.
-usage: python tools/find_bench.py [--mib 512] [--calls 10] [--warmup 3] [--lists-only | --rows-only]"""
+usage: python tools/find_bench.py [--mib 512] [--calls 10] [--warmup 3] [--lists-only | --rows-only | --members-only]"""
 import argparse
 import ctypes as C
 import json
@@ -60,6 +70,7 @@ def main():
     ap.add_argument("--warmup", type=int, default=3)
     ap.add_argument("--lists-only", action="store_true", help="only the list workloads")
     ap.add_argument("--rows-only", action="store_true", help="only the array-rows workloads")
+    ap.add_argument("--members-only", action="store_true", help="only the member-rows workloads")
     args = ap.parse_args()
 
     import numpy as np
@@ -89,6 +100,8 @@ def main():
         return list_rows(args, ctx, L, dev, timed, name, plimit, pk)
     if args.rows_only:
         return array_rows(args, ctx, L, dev, timed, name, plimit)
+    if args.members_only:
+        return member_rows(args, ctx, L, dev, timed, name, plimit, pk)
     lines = pk.split(b"\n")
     keys = [k.encode() for k in json.loads(lines[0])]
     n_rec = (args.mib << 20) // (len(pk) // len(lines) + 1)
@@ -502,6 +515,106 @@ def array_rows(args, ctx, L, dev, timed, name, plimit):
     doc = b"\n".join([lines] * max(1, size // (len(lines) + 1)))
     workload("twitter statuses as NDJSON, ParseND, copy_strings", doc, _lib.FLAG_NDJSON | _lib.FLAG_COPY_STRINGS,
              [b"entities", b"hashtags"], sets([([b"text"], _lib.FIND_KIND_STRING), ([b"indices"], _lib.FIND_KIND_ARRAY_INT64)]))
+    ctx.close()
+
+
+
+def member_rows(args, ctx, L, dev, timed, name, plimit, pk):
+    import torch
+    from simdjson_b200 import _find_paths, _lib
+    from tests.util import load_fixture
+
+    to_dev, parsed, call_timed, marshal_ms = dev_tools(args, ctx, L, dev, timed)
+    i64, u8 = torch.int64, torch.uint8
+
+    def members_call(d_m, mlen, d_t, tw, d_s, slen, row_path, only, paths, kinds):
+        cp, keep = _find_paths(paths, kinds)
+        rp, rkeep = _find_paths([row_path, only], [_lib.FIND_KIND_ELEMENT] * 2)
+        n = [C.c_size_t(0) for _ in range(5)]  # records, rows, bytes, elements, key bytes
+        a = (ctx.h, d_m.data_ptr(), mlen, d_t.data_ptr(), tw, d_s.data_ptr(), slen, rp, C.pointer(rp[1]),
+             cp, len(paths))
+        assert L.sj_find_members_device(*a, None, None, None, None, *(C.byref(x) for x in n)) in (0, _lib.ERR_CAPACITY)
+        N, R, nb, ne, nk = (x.value for x in n)
+        k = len(paths)
+        ns = sum(x in _lib.FIND_VAR_KINDS for x in kinds)
+        o = [torch.empty((k, R), dtype=u8, device=dev), torch.empty((k, R), dtype=u8, device=dev),
+             torch.empty((k, R), dtype=i64, device=dev), torch.empty((k, R), dtype=i64, device=dev),
+             torch.empty((ns, R + 1), dtype=i64, device=dev), torch.empty(max(nb, 1), dtype=u8, device=dev),
+             torch.empty((0, R + 1), dtype=i64, device=dev), torch.empty(1, dtype=i64, device=dev),
+             torch.empty(max(N, 1), dtype=u8, device=dev), torch.empty(N + 1, dtype=i64, device=dev),
+             torch.empty(max(R, 1), dtype=u8, device=dev), torch.empty(max(R, 1), dtype=i64, device=dev),
+             torch.empty(R + 1, dtype=i64, device=dev), torch.empty(max(nk, 1), dtype=u8, device=dev)]
+        out = _lib.FindOut(*(t.data_ptr() for t in o[:6]), R, nb)
+        lo = _lib.FindListsOut(o[6].data_ptr(), o[7].data_ptr(), 0)
+        ro = _lib.FindRowsOut(*(t.data_ptr() for t in o[8:12]), N)
+        ko = _lib.FindKeysOut(o[12].data_ptr(), o[13].data_ptr(), nk)
+
+        def call():
+            assert L.sj_find_members_device(*a, C.byref(out), C.byref(lo), C.byref(ro), C.byref(ko), *(C.byref(x) for x in n)) == 0
+
+        t, launches = call_timed(call)
+        serial = C.c_uint64(0)
+        L.sj_test_find_rows_serial(ctx.h, C.byref(serial))
+        ok = int((o[8][:N] == 0).sum())
+        return t, launches, N, R, nb, nk, serial.value, ok
+
+    def line(label, mlen, tw, words, row_path, only, paths, kinds, res, extra):
+        t, launches, N, R, nb, nk, serial, ok = res
+        ns = sum(x in _lib.FIND_VAR_KINDS for x in kinds)
+        min_bytes = words * 8 + 9 * N + 8 + 9 * R + 8 * (R + 1) + nk + 18 * R * len(paths) + 8 * (R + 1) * ns + nb
+        r = {"input": label, "input_bytes": mlen, "tape_words": tw, "object_words": words,
+             "row_path": [x.decode() for x in row_path], "only_keys": [x.decode() for x in only],
+             "paths": [".".join(x.decode() for x in p) for p in paths], "kinds": list(kinds), "records": N, "records_ok": ok,
+             "rows": R, "key_bytes": nk, "bytes_out": nb, "serial_records": serial, "members_ms": round(t * 1e3, 3),
+             "launches_per_call": launches, "min_bytes": int(min_bytes), "min_gbs": round(min_bytes / t / 1e9, 1),
+             "frac_of_3.35TBs": round(min_bytes / t / 3.35e12, 4),
+             "timer": "CUDA events around %d back-to-back calls after %d warm-up calls" % (args.calls, args.warmup),
+             "card": name, "power_limit_w": plimit}
+        r.update(extra)
+        print(json.dumps(r), flush=True)
+
+    def workload(label, d_m, mlen, flags, row_path, words, runs):
+        d_t, tw, d_s, slen = parsed(d_m, mlen, flags)
+        extra = {"marshal_ms": round(marshal_ms(d_m, mlen, d_t, tw, d_s, slen) * 1e3, 3)}
+        for only, paths, kinds in runs:
+            res = members_call(d_m, mlen, d_t, tw, d_s, slen, row_path, only, paths, kinds)
+            line(label, mlen, tw, words(tw), row_path, only, paths, kinds, res, extra)
+        del d_t, d_s
+        torch.cuda.empty_cache()
+
+    def sets(pk_):
+        return [((), [p], [k]) for p, k in pk_] + [((), [p for p, _ in pk_], [k for _, k in pk_])]
+
+    def one_map(fixture, key):
+        """{key: {...}} of the fixture's map at `key`, its members repeated with unique keys to --mib"""
+        members = list(json.loads(load_fixture(fixture))[key].items())
+        one = [(k, json.dumps(v, separators=(",", ":")).encode()) for k, v in members]
+        size, parts, i, total = args.mib << 20, [], 0, 0
+        while total < size:
+            for k, v in one:
+                p = json.dumps("%s~%d" % (k, i)).encode() + b":" + v
+                parts.append(p)
+                total += len(p) + 1
+            i += 1
+        return b'{"' + key.encode() + b'":{' + b",".join(parts) + b"}}"
+
+    for fixture, key, runs in (("update-center", "plugins", sets([([b"version"], _lib.FIND_KIND_STRING),
+                                                                   ([b"url"], _lib.FIND_KIND_STRING), ([], _lib.FIND_KIND_JSON)])),
+                               ("citm_catalog", "events", sets([([b"name"], _lib.FIND_KIND_STRING), ([], _lib.FIND_KIND_JSON)]))):
+        doc = one_map(fixture, key)
+        d_m = to_dev(doc)
+        workload("{\"%s\": %s's %s with unique keys x k}, Parse, copy_strings" % (key, fixture, key), d_m, len(doc),
+                 _lib.FLAG_COPY_STRINGS, [key.encode()], lambda tw: tw - 6, runs)
+        del d_m
+    lines = pk.split(b"\n")
+    keys = [k.encode() for k in json.loads(lines[0])]
+    n_rec = (args.mib << 20) // (len(pk) // len(lines) + 1)
+    d_m = torch.full(((args.mib << 20) + (4 << 20),), 0x20, dtype=torch.uint8, device=dev)
+    glen = C.c_size_t(0)
+    assert L.sj_gen_ndjson_device(ctx.h, pk, len(pk), 0, n_rec, d_m.data_ptr(), d_m.numel() - (1 << 16), C.byref(glen)) == 0
+    workload("K0 batch (parking citations), ParseND, copy_strings", d_m, glen.value, _lib.FLAG_NDJSON | _lib.FLAG_COPY_STRINGS,
+             [], lambda tw: tw - 2 * n_rec, [((), [[]], [_lib.FIND_KIND_STRING_CVT]),
+                                             ((keys[1], keys[5]), [[]], [_lib.FIND_KIND_STRING_CVT])])
     ctx.close()
 
 

@@ -100,6 +100,26 @@ k = int(fr.find_rows(tape_r, str_r, b"", [b"a"], [], [])[3][1])  # the head of t
 nop[k], nop[k + 1] = (ord("N") << 56) | 1, 0  # a nop over the number: its record is walked by one thread
 rc, N, R, index, _ = ctx.find_rows_device(torch.from_numpy(nop.view(np.int64).copy()).cuda(), s_r, m_r, [b"a"], rpaths, rkinds)
 assert rc == 0 and ctx.find_rows_serial() == 1
+# the find's member rows (KO1 .. KO4 with the array rows' passes), on the own tape and a foreign copy, with only_keys
+# and with a nop between a key and its value so that one record takes the one-thread walk
+from tests import find_members_oracle as fmo
+
+for rp, only in (([b"a"], []), ([], [b"a", b"b"])):
+    want_m = fmo.find_members(tape_r, str_r, rdoc[off_r:off_r + len_r], rp, [[]], [7], only)
+    rc, N, R, index, _ = ctx.parse_find_members(rdoc, rp, [[]], [7], only)
+    assert rc == 0 and index.row_index.tolist() == want_m[3], (rp, index.row_index, want_m[3])
+    rc, N, R, index, _ = ctx.find_members_device(t_r, s_r, m_r, rp, [[]], [7], only)
+    assert rc == 0 and index.row_index.cpu().tolist() == want_m[3]
+mdoc = b'{"a":{"k":1,"s":"x"},"b":2}'
+rc_o, tape_m, str_m, (off_m, len_m) = o.parse(mdoc)
+nop = np.insert(tape_m, 7, np.uint64(ord("N") << 56))  # a nop between "k" and its value (skip 0)
+scope = np.isin(nop >> np.uint64(56), [ord(c) for c in "r{}"]) & ((nop & np.uint64((1 << 56) - 1)) >= 7)
+nop[scope] += np.uint64(1)
+rc, N, R, index, _ = ctx.find_members_device(torch.from_numpy(nop.view(np.int64).copy()).cuda(),
+                                             torch.frombuffer(bytearray(str_m), dtype=torch.uint8).cuda(),
+                                             torch.frombuffer(bytearray(mdoc[off_m:off_m + len_m]), dtype=torch.uint8).cuda(),
+                                             [b"a"], [[]], [1])
+assert rc == 0 and R == 2 and ctx.find_rows_serial() == 1
 # the S2 blocks of CompressFast (s2.cuh): KC1 / KC2 and KX1 / KX2 around the same calls
 from tests import s2_oracle
 ctx.set_compress_mode(1)
